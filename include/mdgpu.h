@@ -305,6 +305,20 @@ int mdgpu_plan_property_aggregate(mdgpu_plan* plan, size_t prop, float* out_mean
  * receives counts scaled by 1 / (bin width x samples of the row), out_min_max (optional) the smallest / largest scaled bin. Implies mdgpu_plan_sync. */
 int mdgpu_plan_property_histogram(mdgpu_plan* plan, size_t prop, uint32_t num_bins, float range_min, float range_max, int aggregate, float* out_bins, float* out_min_max);
 
+/* VIAMD's Ramachandran density (src/components/ramachandran/ramachandran.cpp:1277-1370, rama_rep_compute_density) from the (phi, psi) rows of an
+ * MDGPU_OP_BACKBONE_ANGLES property, on the device. Class c (0 general, 1 glycine, 2 proline, 3 pre-proline: segment.rama_type as
+ * md_util_backbone_ramachandran_classify fills it) holds the segments segments[class_offsets[c] .. class_offsets[c+1]). Every frame of
+ * [frame_beg, frame_end) that has been evaluated (frame-mask bit set) and every listed segment whose angles are not (0, 0) adds 1 to texel (x, y)
+ * of channel c, then the map is blurred by three box passes per axis with the radii of boxes_for_gauss(., 3, sigma) (blur_density_gaussian :368-387).
+ * out_tex[512][512][4] receives the map in VIAMD's density_tex layout (texel y * 512 + x, RGBA = the four classes), out_sum[c] the samples of class c.
+ * sigma must lie in VIAMD's slider range [0.1, 10]. Implies mdgpu_plan_sync; runs on devices[0] of a multi-device plan.
+ * Numerical contract (against the reference built with -fno-fast-math -ffp-contract=off): u = phi * s + 0.5f and v = psi * s + 0.5f with
+ * s = (float)(1 / 2pi) and two roundings each, x = ((uint32_t)(u * 512.0f)) & 511 truncating toward zero (phi = -pi lands in texel 0, phi = pi wraps
+ * to 0), the same for y; a texel's value is min(samples, 2^24), the exact result of adding 1.0f per sample in float; the box passes add and subtract
+ * in the reference's order, so the map equals the reference's value for value (only the sign of a zero may differ); out_sum[c] = (float)(double)n. */
+int mdgpu_plan_rama_density(mdgpu_plan* plan, size_t prop, const uint32_t* segments, const uint32_t class_offsets[5], uint32_t frame_beg, uint32_t frame_end,
+                            float sigma, float* out_tex, float out_sum[4]);
+
 /* Exact integer results (what parity is asserted on).
  *  _counts: accumulated counts over all evaluated frames: RDF 1024 x u64 bins; SDF 128^3 x u64 voxels (widened from u32);
  *           DENSITY 1024 x u64 fixed-point mass sums (unit 2^-24 Da).

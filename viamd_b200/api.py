@@ -623,6 +623,25 @@ class Plan:
         _check(lib().mdgpu_plan_property_histogram(self._h, i, num_bins, range_min, range_max, 1 if aggregate else 0, out.ctypes.data, mm.ctypes.data))
         return out, (float(mm[0]), float(mm[1]))
 
+    def rama_density(self, name, classes, frame_beg: int = 0, frame_end: Optional[int] = None, sigma: float = 5.0):
+        """VIAMD's Ramachandran density maps (rama_rep_compute_density) from the backbone-angles property `name`, computed on the device over the
+        evaluated frames of [frame_beg, frame_end). classes: four arrays of segment indices (general, glycine, proline, pre-proline).
+        Returns (tex [512, 512, 4] float32 indexed [y, x, class], sums [4] float32 samples per class)."""
+        i = self._index(name)
+        if len(classes) != 4:
+            raise ValueError("classes: four arrays of segment indices (general, glycine, proline, pre-proline)")
+        lists = [np.ascontiguousarray(c, np.int64).ravel() for c in classes]
+        if any(len(c) and (c.min() < 0 or c.max() > 0xFFFFFFFF) for c in lists):
+            raise ValueError("classes: segment indices must be non-negative 32-bit integers")
+        seg = np.ascontiguousarray(np.concatenate(lists), np.uint32)
+        off = np.zeros(5, np.uint32); off[1:] = np.cumsum([len(c) for c in lists])
+        tex = np.zeros((512, 512, 4), np.float32); sums = np.zeros(4, np.float32)
+        end = self.num_frames if frame_end is None else int(frame_end)
+        L = lib(); L.mdgpu_plan_rama_density.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_float, C.c_void_p, C.c_void_p]
+        _check(L.mdgpu_plan_rama_density(self._h, i, seg.ctypes.data if seg.size else None, off.ctypes.data, int(frame_beg), end, float(sigma),
+                                          tex.ctypes.data, sums.ctypes.data))
+        return tex, sums
+
     def exchange_stats(self):
         ms = C.c_double(); n = C.c_uint64(); _check(lib().mdgpu_plan_exchange_stats(self._h, C.byref(ms), C.byref(n))); return ms.value, int(n.value)
 

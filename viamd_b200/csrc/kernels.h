@@ -149,6 +149,21 @@ void launch_temporal_histogram(const float* d_values, const unsigned long long* 
                                uint32_t num_bins, int aggregate, uint32_t* d_counts, uint32_t* d_totals, cudaStream_t s);
 void launch_mean_u32(const uint32_t* d_in, float* d_out, size_t count, unsigned long long n, cudaStream_t s);
 
+// rama.cu — VIAMD's Ramachandran density maps from the (phi, psi) rows of a backbone-angles temporal
+struct RamaArgs {
+    const float* angles; uint32_t n_seg;         // [num_frames][n_seg][2]
+    const uint32_t* seg; uint32_t n_entries;      // the class lists back to back: segment index per entry
+    uint32_t class_end[3];                        // entries [0, class_end[0]) are class 0, ... [class_end[2], n_entries) class 3
+    uint32_t frame_beg, frame_count; const unsigned long long* mask;   // frames [beg, beg + count) whose mask bit is set
+    float scale;                                  // (float)(1 / 2pi): angle -> texture coordinate
+    unsigned long long* counts;                   // [512][512][4] scratch (element (x, y, c) at (x * 512 + y) * 4 + c)
+    unsigned long long* samples;                  // [4] samples per class
+    float* buf[3];                                // [512][512][4] float scratch each; the blurred map ends in buf[1] as [y][x][c]
+    int box[3];                                   // box radii of the three passes per axis (boxes_for_gauss)
+    int sm_count;
+};
+void launch_rama_density(const RamaArgs& a, cudaStream_t s);
+
 // xtc.cu — compressed trajectory frames expanded on the device
 struct XtcFrameInfo {   // written by k_xtc_scan, one per frame
     int status;                 // 0 ok, otherwise the frame is malformed

@@ -89,6 +89,7 @@ struct Prop {
     uint32_t* d_set_of = nullptr;   // contact_count: set of every atom of the concatenated A list
     int share_trg = -1;   // index of an earlier property with the same target selection and cutoff: its target cell list is reused
     size_t trg_groups = 0;   // rdf: the target argument was an ARRAY of selections: one centre of mass per selection is the target point (h_goff[1] = their CSR offsets in idx[1])
+    size_t backbone_segments = 0;   // MDGPU_OP_BACKBONE_ANGLES (evaluated as 2 dihedrals in context per segment): the segments of its (phi, psi) rows
 };
 
 struct PropScratch {   // per (stream slot, property)
@@ -649,7 +650,7 @@ mdgpu_plan* mdgpu_plan_create(const mdgpu_system_desc_t* sys, const mdgpu_proper
                 cudaFree(pr.d_idx[k]); pr.d_idx[k] = nullptr; pr.h_idx[k] = ctx[k];
                 if (upload(&pr.d_idx[k], pr.h_idx[k].data(), pr.h_idx[k].size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (indices)");
             }
-            pr.op = MDGPU_OP_DIHEDRAL; pr.n_struct = 2 * ns; pr.len = 2 * ns;
+            pr.op = MDGPU_OP_DIHEDRAL; pr.n_struct = 2 * ns; pr.len = 2 * ns; pr.backbone_segments = ns;
             e = dalloc(&pr.d_temporal, num_frames * pr.len);
             pr.values.assign(num_frames * pr.len, 0.0f);
             pr.agg_mean.assign(num_frames, 0.0f); pr.agg_var.assign(num_frames, 0.0f); pr.agg_ext.assign(2 * num_frames, 0.0f);
@@ -1836,6 +1837,54 @@ int mdgpu_plan_property_histogram(mdgpu_plan* p, size_t prop, uint32_t num_bins,
         for (uint32_t j = 0; j < num_bins; ++j) { float v = (float)counts[(size_t)i * num_bins + j]; v *= scl; out_bins[(size_t)i * num_bins + j] = v; min_bin = std::min(min_bin, v); max_bin = std::max(max_bin, v); }
     }
     if (out_min_max) { out_min_max[0] = min_bin; out_min_max[1] = max_bin; }
+    return done(0);
+}
+
+// Radii of the three box passes per axis that approximate a Gaussian of `sigma` texels: boxes_for_gauss(., 3, sigma) of VIAMD's Ramachandran
+// component (src/components/ramachandran/ramachandran.cpp:333-344), with the same float expressions so that the radii agree for every sigma.
+static void rama_box_radii(int r[3], float sigma) {
+    const float ideal = sqrtf(12 * sigma * sigma / 3 + 1);                                  // ideal width of one of three boxes
+    int lo = (int)ideal; if (lo % 2 == 0) --lo;                                              // the odd width at or below it
+    const float passes_lo = (12 * sigma * sigma - 3 * lo * lo - 12 * lo - 9) / (-4 * lo - 4);   // how many passes use lo, the rest lo + 2
+    const int n_lo = (int)(passes_lo + 0.5f);
+    for (int i = 0; i < 3; ++i) r[i] = i < n_lo ? lo : lo + 2;
+}
+
+int mdgpu_plan_rama_density(mdgpu_plan* p, size_t prop, const uint32_t* segments, const uint32_t class_offsets[5], uint32_t frame_beg, uint32_t frame_end,
+                            float sigma, float* out_tex, float out_sum[4]) {
+    if (!p || prop >= p->props.size() || !class_offsets || !out_tex || !out_sum) return fail(MDGPU_ERR_INVALID_ARG, "mdgpu_plan_rama_density: invalid argument");
+    Prop& pr = p->props[prop];
+    if (!pr.backbone_segments) return fail(MDGPU_ERR_INVALID_ARG, "property '%s' is not a backbone-angles property", pr.name.c_str());
+    for (int c = 0; c < 4; ++c) if (class_offsets[c] > class_offsets[c + 1]) return fail(MDGPU_ERR_INVALID_ARG, "mdgpu_plan_rama_density: class offsets decrease");
+    const uint32_t n_entries = class_offsets[4] - class_offsets[0];
+    if (n_entries && !segments) return fail(MDGPU_ERR_INVALID_ARG, "mdgpu_plan_rama_density: no segment list");
+    for (uint32_t e = class_offsets[0]; e < class_offsets[4]; ++e)
+        if (segments[e] >= pr.backbone_segments) return fail(MDGPU_ERR_INVALID_ARG, "mdgpu_plan_rama_density: segment %u out of range (%zu segments)", segments[e], pr.backbone_segments);
+    if (frame_beg > frame_end || frame_end > p->num_frames) return fail(MDGPU_ERR_INVALID_ARG, "mdgpu_plan_rama_density: frame range [%u, %u) outside [0, %zu)", frame_beg, frame_end, p->num_frames);
+    // VIAMD's blur slider range; it keeps every box radius far below 256, which the wrap of the box passes assumes
+    if (!(sigma >= 0.1f && sigma <= 10.0f)) return fail(MDGPU_ERR_INVALID_ARG, "mdgpu_plan_rama_density: sigma %g outside [0.1, 10]", (double)sigma);
+    int rc = mdgpu_plan_sync(p); if (rc) return rc;   // multi-device plans hold every frame's rows on devices[0] = p->device from here on
+    CUDA_TRY(cudaSetDevice(p->device));
+    std::vector<uint64_t> mask; { std::lock_guard<std::mutex> lk(p->mask_mutex); mask = p->frame_mask; }
+    const size_t texels = 512 * 512 * 4;
+    RamaArgs a{};
+    unsigned long long* d_mask = nullptr; uint32_t* d_seg = nullptr; unsigned long long* d_counts = nullptr; unsigned long long* d_samples = nullptr; float* d_buf = nullptr;
+    auto done = [&](int r) { cudaFree(d_mask); cudaFree(d_seg); cudaFree(d_counts); cudaFree(d_samples); cudaFree(d_buf); return r; };
+    if (dalloc(&d_mask, mask.size()) != cudaSuccess || upload(&d_seg, segments ? segments + class_offsets[0] : nullptr, n_entries) != cudaSuccess ||
+        dalloc(&d_counts, texels) != cudaSuccess || dalloc(&d_samples, 4) != cudaSuccess || dalloc(&d_buf, 3 * texels) != cudaSuccess)
+        return done(fail(MDGPU_ERR_CUDA, "device allocation failed (rama density)"));
+    if (cudaMemcpy(d_mask, mask.data(), sizeof(uint64_t) * mask.size(), cudaMemcpyHostToDevice) != cudaSuccess) return done(fail(MDGPU_ERR_CUDA, "frame mask upload failed (rama density)"));
+    a.angles = pr.d_temporal; a.n_seg = (uint32_t)pr.backbone_segments; a.seg = d_seg; a.n_entries = n_entries;
+    for (int c = 0; c < 3; ++c) a.class_end[c] = class_offsets[c + 1] - class_offsets[0];
+    a.frame_beg = frame_beg; a.frame_count = frame_end - frame_beg; a.mask = d_mask;
+    a.scale = (float)(1.0 / (2.0 * 3.1415926535897932));   // 1.0f / (2.0f * PI) with the double PI of md_common.h:157
+    a.counts = d_counts; a.samples = d_samples; a.buf[0] = d_buf; a.buf[1] = d_buf + texels; a.buf[2] = d_buf + 2 * texels;
+    rama_box_radii(a.box, sigma); a.sm_count = p->sm_count;
+    launch_rama_density(a, 0);
+    uint64_t samples[4] = { 0, 0, 0, 0 };
+    if (cudaMemcpy(out_tex, a.buf[1], sizeof(float) * texels, cudaMemcpyDeviceToHost) != cudaSuccess || cudaMemcpy(samples, d_samples, sizeof(samples), cudaMemcpyDeviceToHost) != cudaSuccess)
+        return done(fail(MDGPU_ERR_CUDA, "rama density failed: %s", cudaGetErrorString(cudaGetLastError())));
+    for (int c = 0; c < 4; ++c) out_sum[c] = (float)(double)samples[c];   // den_sum: (float) of the task's double sum
     return done(0);
 }
 
