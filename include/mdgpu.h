@@ -86,6 +86,8 @@ typedef struct mdgpu_system_desc_t {
     const uint32_t* bond_conn_offset;  /* [bond_conn_offset_count] (= num_atoms + 1), may be NULL if no sdf / rmsd property */
     const int32_t* bond_conn_atom_idx;
     size_t bond_conn_offset_count;
+    const float* atom_radius;          /* [num_atoms] van der Waals radii as md_atom_extract_radii(r, 0, num_atoms, &sys->atom) gives them; may be NULL
+                                        * unless a property is MDGPU_OP_POROSITY (mdgpu_plan_create then fails with MDGPU_ERR_INVALID_ARG) */
 } mdgpu_system_desc_t;
 
 /* Property operations (the procedures[] entries on the hot path, md_script_functions.inl:574-730). */
@@ -111,6 +113,7 @@ typedef enum mdgpu_op {
     MDGPU_OP_CONTACT_COUNT = 21, /* contact_count(A[], B, cutoff) -> temporal [F, |A|]; exclusion lists from the caller :2756-2866 */
     MDGPU_OP_BACKBONE_ANGLES = 20, /* (phi, psi) of every backbone segment per frame -> temporal [F, 2 * n_segments]: VIAMD's "Backbone Operations" pass
                                     * (src/viamd.cpp:488-520 -> md_util_backbone_angles_compute md_util.c:2572-2620) */
+    MDGPU_OP_POROSITY = 22,  /* porosity(selection): unoccupied fraction of a voxel grid over the selection's van der Waals spheres -> temporal [F, 1] :5858-6003 */
 } mdgpu_op;
 
 /* One property = one `ident = proc(args);` statement whose selections were evaluated statically at compile time
@@ -150,6 +153,20 @@ typedef enum mdgpu_op {
  *              md_util.c:2588-2592) whose two values stay 0. Row f holds md_backbone_angles_t[num_structures] = (phi, psi) pairs in radians:
  *              phi = dihedral(C', N, CA, C), psi = dihedral(N, CA, C, N') with md_util_min_image_vec3 on the bond vectors, as `dihedral` evaluates.
  *   RMSD     : idx[0] = the atoms of the (flattened) selection; needs the initial frame and, to make molecules whole, the bond connectivity.
+ *   POROSITY : idx[0] = the atoms of the (flattened) selection, ascending; needs mdgpu_system_desc_t.atom_radius. Per frame, value_range [0, 1]:
+ *              0 when the frame's cell is triclinic or the selection is empty (as the reference, which logs an error there). Otherwise
+ *              xyzr = (x, y, z, radius) of the selected atoms in index order; com = md_util_com_compute_vec4(xyzr, 0, n, cell) (the trigonometric
+ *              centre of mass weighted by the radii: serial float sums in index order); md_util_deperiodize_vec4 about com; bmin / bmax = min(p - r) /
+ *              max(p + r) per axis; ext = max(bmax - bmin, 1.0f), t = max(ext) / 512 (exact), dim = max(1, (int)(ext / t)) (the longest axis gets
+ *              512), d = ext / (float)dim. A sphere covers the voxels of the index box (int)floorf(((p -+ r) - bmin) / d) clamped to [0, dim - 1] whose
+ *              centre c = bmin + ((float)i + 0.5f) * d passes fmaf(dx, dx, fmaf(dy, dy, dz * dz)) <= r * r with d* = c - p; those two fmaf are the only
+ *              fused operations, everything else rounds separately. With `set` occupied voxels out of N = dim0 * dim1 * dim2, the value is 0 if
+ *              set == 0, else (float)(((double)N - set) / (double)N). mdgpu_plan_property_frame_rows gives set (which = 0) and N (which = 1) per
+ *              frame as u64, zero for frames not evaluated. Values equal the reference's wherever it is defined: the reference weights the centre of
+ *              mass and pads the box with rad[atom index] from an array that holds only the radii of atoms 0 .. n-1 (md_atom_extract_radii(rad, 0,
+ *              count) :5906, read through extract_xyzw_vec4 :5912), which is correct only when the selection is a prefix of the atoms (all,
+ *              atom(1:k), residue(1:k)) and reads past the array otherwise; the library uses each selected atom's own radius, as the reference's voxel
+ *              loop does (:5946). N <= 2^23 makes the float value determine `set` uniquely; larger grids can share a value between counts.
  *   DISTANCE/ANGLE/DIHEDRAL: idx[k] = the atoms of argument k (0-based). A single integer index is that atom's position; an
  *              argument that was a selection (bit k of com_args set, or more than one index) is its centre of mass as
  *              coordinate_extract_com evaluates it (:1717 -> md_util_com_compute md_util.c:8163: periodic cells use the

@@ -24,7 +24,7 @@ LIB_PATH = os.path.join(HERE, "libmdgpu.so")
 DIST_BINS = 1024
 VOL_DIM = 128
 
-OP_RDF, OP_SDF, OP_DENSITY_X, OP_DENSITY_Y, OP_DENSITY_Z, OP_DISTANCE, OP_ANGLE, OP_DIHEDRAL, OP_DISTANCE_MIN, OP_DISTANCE_MAX, OP_RMSD, OP_DISTANCE_PAIR, OP_COM, OP_PLANE, OP_WITHIN_COUNT, OP_SHAPE_WEIGHTS, OP_COORD_X, OP_COORD_Y, OP_COORD_Z, OP_BACKBONE_ANGLES, OP_CONTACT_COUNT = 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16, 17, 18, 19, 20, 21
+OP_RDF, OP_SDF, OP_DENSITY_X, OP_DENSITY_Y, OP_DENSITY_Z, OP_DISTANCE, OP_ANGLE, OP_DIHEDRAL, OP_DISTANCE_MIN, OP_DISTANCE_MAX, OP_RMSD, OP_DISTANCE_PAIR, OP_COM, OP_PLANE, OP_WITHIN_COUNT, OP_SHAPE_WEIGHTS, OP_COORD_X, OP_COORD_Y, OP_COORD_Z, OP_BACKBONE_ANGLES, OP_CONTACT_COUNT, OP_POROSITY = 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16, 17, 18, 19, 20, 21, 22
 CELL_ORTHO, CELL_TRICLINIC, CELL_PBC_X, CELL_PBC_Y, CELL_PBC_Z, CELL_PBC_ALL = 1, 2, 4, 8, 16, 28
 
 
@@ -63,7 +63,8 @@ class FrameHeader(C.Structure):
 
 class _SystemDesc(C.Structure):
     _fields_ = [("num_atoms", C.c_size_t), ("atom_mass", C.POINTER(C.c_float)), ("bond_conn_offset", C.POINTER(C.c_uint32)),
-                ("bond_conn_atom_idx", C.POINTER(C.c_int32)), ("bond_conn_offset_count", C.c_size_t)]
+                ("bond_conn_atom_idx", C.POINTER(C.c_int32)), ("bond_conn_offset_count", C.c_size_t),
+                ("atom_radius", C.POINTER(C.c_float))]
 
 
 class _DynArg(C.Structure):   # mdgpu_dynamic_arg_t
@@ -207,6 +208,7 @@ class System:
     name: Optional[Sequence[str]] = None
     resname: Optional[Sequence[str]] = None        # per residue
     res_atom_offset: Optional[np.ndarray] = None   # [num_res + 1]
+    radius: Optional[np.ndarray] = None            # van der Waals radii (md_atom_extract_radii); required by porosity()
 
 
 @dataclass
@@ -447,6 +449,12 @@ def rmsd(name, idx):
     return Property(name, OP_RMSD, [np.asarray(idx, np.int32)])
 
 
+def porosity(name, idx):
+    """porosity(selection): per frame, the unoccupied fraction of a bit grid (longest axis 512 voxels) over the bounding box of the selection's van
+    der Waals spheres (_porosity md_script_functions.inl:5858). Needs System.radius. 0 for a triclinic cell or an empty selection."""
+    return Property(name, OP_POROSITY, [np.asarray(idx, np.int32)])
+
+
 def angle(name, a, b, c):
     return _temporal(name, OP_ANGLE, (a, b, c))
 
@@ -550,6 +558,10 @@ class Plan:
             co = np.ascontiguousarray(system.conn_offset, np.uint32); ci = np.ascontiguousarray(system.conn_idx, np.int32); self._keep += [co, ci]
             sd.bond_conn_offset = co.ctypes.data_as(C.POINTER(C.c_uint32)); sd.bond_conn_atom_idx = ci.ctypes.data_as(C.POINTER(C.c_int32))
             sd.bond_conn_offset_count = len(co)
+        if system.radius is not None:
+            rad = np.ascontiguousarray(system.radius, np.float32); self._keep.append(rad)
+            if rad.shape != (system.num_atoms,): raise ValueError("System.radius: one radius per atom expected")
+            sd.atom_radius = rad.ctypes.data_as(C.POINTER(C.c_float))
         descs = (_PropertyDesc * len(self.properties))()
         for i, p in enumerate(self.properties):
             d = descs[i]; nm = p.name.encode(); self._keep.append(nm)

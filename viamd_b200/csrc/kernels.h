@@ -1,4 +1,4 @@
-// kernels.h — host-callable launchers of the per-batch kernels (defined in cells.cu, rdf.cu, sdf.cu, props.cu, synth.cu)
+// kernels.h — host-callable launchers of the per-batch kernels (defined in cells.cu, rdf.cu, sdf.cu, props.cu, porosity.cu, synth.cu)
 #pragma once
 #include "common.cuh"
 
@@ -163,6 +163,31 @@ struct RamaArgs {
     int sm_count;
 };
 void launch_rama_density(const RamaArgs& a, cudaStream_t s);
+
+// porosity.cu — porosity(selection): the unoccupied fraction of a 512-voxel bit grid over the selection's van der Waals spheres, per frame
+constexpr uint32_t PORO_FRAMES = 8;                         // frames per sub-batch: one grid each, per stream slot
+constexpr size_t PORO_GRID_WORDS = (size_t)8 * 512 * 512;   // the largest grid: ceil(512 / 64) words per row x 512 x 512 rows (16 MiB)
+struct PorosityHdr {                 // per frame, written by k_porosity_prepare
+    float bmin[3], d[3];             // box minimum, voxel size per axis
+    int dim[3];                      // voxels per axis; the longest axis has 512
+    uint32_t row_words;              // 64-bit words per grid row, ceil(dim[0] / 64)
+    uint32_t valid;                  // 0: triclinic cell or empty selection, the value is 0
+};
+struct PorosityArgs {
+    BatchFrames frames;              // the sub-batch: at most PORO_FRAMES frames
+    const mdgpu_unitcell_t* cells;   // [frames.count]
+    const int32_t* idx; uint32_t n;  // the selection's atoms, ascending
+    const float* radius;             // [atoms] van der Waals radii in the frames' atom space
+    float4* xyzr;                    // [PORO_FRAMES][n] scratch
+    PorosityHdr* hdr;                // [PORO_FRAMES]
+    unsigned long long* grid;        // [PORO_FRAMES][PORO_GRID_WORDS], all zero between calls
+    unsigned long long* count;       // [PORO_FRAMES], all zero between calls
+    unsigned long long* frame_set;   // [num_frames] occupied voxels
+    unsigned long long* frame_n;     // [num_frames] voxels of the grid (N)
+    float* out;                      // [num_frames]
+    uint32_t frame0;                 // global index of the sub-batch's first frame
+};
+void launch_porosity(const PorosityArgs& a, int nf, cudaStream_t s);
 
 // xtc.cu — compressed trajectory frames expanded on the device
 struct XtcFrameInfo {   // written by k_xtc_scan, one per frame

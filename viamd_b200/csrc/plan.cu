@@ -90,6 +90,7 @@ struct Prop {
     int share_trg = -1;   // index of an earlier property with the same target selection and cutoff: its target cell list is reused
     size_t trg_groups = 0;   // rdf: the target argument was an ARRAY of selections: one centre of mass per selection is the target point (h_goff[1] = their CSR offsets in idx[1])
     size_t backbone_segments = 0;   // MDGPU_OP_BACKBONE_ANGLES (evaluated as 2 dihedrals in context per segment): the segments of its (phi, psi) rows
+    unsigned long long* d_frame_n = nullptr;   // porosity: voxels of each frame's grid (N); d_frame_total holds the occupied ones
 };
 
 struct PropScratch {   // per (stream slot, property)
@@ -107,6 +108,8 @@ struct PropScratch {   // per (stream slot, property)
     // rdf candidate lists (k_rdf_cull): [B][list_stride] entries, [B][cap] headers, [B] cursors
     uint32_t* d_pair_list = nullptr; uint4* d_list_hdr = nullptr; uint32_t* d_list_cursor = nullptr; size_t list_stride = 0;
     mdgpu_unitcell_t nn_cell{}; size_t nn_of_cell = 0; bool nn_valid = false;   // neighbour-offset count of the last cell seen (list sizing)
+    // porosity: per sub-batch of PORO_FRAMES frames the spheres, grid headers, bit grids (zero between sub-batches) and occupied-voxel counters
+    float4* d_poro_xyzr = nullptr; PorosityHdr* d_poro_hdr = nullptr; unsigned long long* d_poro_grid = nullptr; unsigned long long* d_poro_count = nullptr;
 };
 
 struct Slot {
@@ -171,6 +174,7 @@ struct mdgpu_plan {
     size_t num_atoms = 0, num_frames = 0; size_t axis_stride = 0;   // staging layout: [frame][3][axis_stride]
     uint32_t B = 132; uint32_t S = 2; uint32_t cell_cap = 0; bool keep = false; uint32_t rdf_variant = 0;
     std::vector<float> h_mass; float* d_mass = nullptr;
+    std::vector<float> h_radius; float* d_radius = nullptr; float* d_radius_c = nullptr;   // van der Waals radii (porosity plans only)
     // Compact atom space: the union of the atoms any property reads, ascending. When it is well below the system size, host ingest copies
     // only those atoms (gathered into pinned staging by the ingest threads) and the kernels run on index lists remapped into that space.
     bool compact = false; std::vector<int32_t> needed; size_t num_atoms_c = 0, axis_stride_c = 0; float* d_mass_c = nullptr; float* d_init_c = nullptr;
@@ -302,6 +306,7 @@ static void destroy_plan(mdgpu_plan* p) {
         for (auto& ps : s.ps) {
             cudaFree(ps.d_geom); cudaFree(ps.d_aabb); free_cell_list(ps.trg); free_cell_list(ps.ref);
             cudaFree(ps.d_frame_bins); cudaFree(ps.d_frame_bins64); cudaFree(ps.d_sdf_xyzw); cudaFree(ps.d_sdf_ref0); cudaFree(ps.d_sdf_mats); cudaFree(ps.d_com); cudaFree(ps.d_argpos); cudaFree(ps.d_gpos[0]); cudaFree(ps.d_gpos[1]); for (auto* q : ps.d_parts) cudaFree(q); cudaFree(ps.d_flags); for (auto& w : ps.dynw) { cudaFree(w.d_geom); cudaFree(w.d_aabb); free_cell_list(w.trg); free_cell_list(w.ref); cudaFree(w.d_flags); cudaFree(w.d_idx); cudaFree(w.d_n); } cudaFree(ps.d_pair_list); cudaFree(ps.d_list_hdr); cudaFree(ps.d_list_cursor);
+            cudaFree(ps.d_poro_xyzr); cudaFree(ps.d_poro_hdr); cudaFree(ps.d_poro_grid); cudaFree(ps.d_poro_count);
         }
         cudaFree(s.d_frames); if (s.h_frames) cudaFreeHost(s.h_frames); cudaFree(s.d_xtc_frames);
         cudaFree(s.d_cells); if (s.h_cells) cudaFreeHost(s.h_cells); cudaFree(s.d_err);
@@ -322,12 +327,12 @@ static void destroy_plan(mdgpu_plan* p) {
         if (pr.values_registered) cudaHostUnregister(pr.values.data());
         cudaFree(pr.d_vol_mean);
         cudaFree(pr.d_acc); cudaFree(pr.d_vol); cudaFree(pr.d_frame_total); cudaFree(pr.d_frame_min); cudaFree(pr.d_frame_max);
-        cudaFree(pr.d_frame_min64); cudaFree(pr.d_frame_max64); cudaFree(pr.d_keep); cudaFree(pr.d_keep64); cudaFree(pr.d_temporal); cudaFree(pr.d_unwrap); cudaFree(pr.d_soff); cudaFree(pr.d_and_mask); cudaFree(pr.d_goff[0]); cudaFree(pr.d_goff[1]); for (auto* q : pr.d_aoff) cudaFree(q); cudaFree(pr.d_set_of); for (auto& dy : pr.dyn) cudaFree(dy.d_and_mask);
+        cudaFree(pr.d_frame_min64); cudaFree(pr.d_frame_max64); cudaFree(pr.d_keep); cudaFree(pr.d_keep64); cudaFree(pr.d_temporal); cudaFree(pr.d_unwrap); cudaFree(pr.d_soff); cudaFree(pr.d_and_mask); cudaFree(pr.d_goff[0]); cudaFree(pr.d_goff[1]); for (auto* q : pr.d_aoff) cudaFree(q); cudaFree(pr.d_set_of); for (auto& dy : pr.dyn) cudaFree(dy.d_and_mask); cudaFree(pr.d_frame_n);
     }
     for (auto& t : p->timed) { cudaEventDestroy(t.a); cudaEventDestroy(t.b); }
     if (p->t_begin) cudaEventDestroy(p->t_begin);
     for (auto e : p->t_end) cudaEventDestroy(e);
-    cudaFree(p->d_mass); cudaFree(p->d_init); cudaFree(p->d_mass_c); cudaFree(p->d_init_c); cudaFree(p->d_counters);
+    cudaFree(p->d_mass); cudaFree(p->d_radius); cudaFree(p->d_radius_c); cudaFree(p->d_init); cudaFree(p->d_mass_c); cudaFree(p->d_init_c); cudaFree(p->d_counters);
     delete p->pool;
     delete p;
 }
@@ -414,6 +419,13 @@ mdgpu_plan* mdgpu_plan_create(const mdgpu_system_desc_t* sys, const mdgpu_proper
         return std::string();
     };
     if (upload(&p->d_mass, p->h_mass.data(), p->h_mass.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (masses)");
+    for (size_t i = 0; i < num_props; ++i) if (props[i].op == MDGPU_OP_POROSITY) {   // porosity voxelises van der Waals spheres: the radii are required
+        if (!sys->atom_radius) return bail(MDGPU_ERR_INVALID_ARG, "porosity: the system description has no atom radii (mdgpu_system_desc_t.atom_radius)");
+        p->h_radius.assign(sys->atom_radius, sys->atom_radius + sys->num_atoms);
+        for (size_t a = 0; a < sys->num_atoms; ++a) if (!(p->h_radius[a] >= 0.0f && p->h_radius[a] <= FLT_MAX)) return bail(MDGPU_ERR_INVALID_ARG, "porosity: atom radius " + std::to_string(a) + " is negative or not finite");
+        if (upload(&p->d_radius, p->h_radius.data(), p->h_radius.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (radii)");
+        break;
+    }
 
     p->props.resize(num_props);
     for (size_t i = 0; i < num_props; ++i) {
@@ -656,6 +668,13 @@ mdgpu_plan* mdgpu_plan_create(const mdgpu_system_desc_t* sys, const mdgpu_proper
             pr.agg_mean.assign(num_frames, 0.0f); pr.agg_var.assign(num_frames, 0.0f); pr.agg_ext.assign(2 * num_frames, 0.0f);
             pr.data.dim[0] = (int32_t)num_frames; pr.data.dim[1] = (int32_t)pr.len; pr.data.dim[2] = 0; pr.data.dim[3] = 0;
             break; }
+        case MDGPU_OP_POROSITY:   // porosity(selection): [F, 1]; an empty selection is valid and evaluates to 0 (:5896-5899)
+            e = dalloc(&pr.d_temporal, num_frames);
+            if (e == cudaSuccess) e = dalloc(&pr.d_frame_total, num_frames);
+            if (e == cudaSuccess) e = dalloc(&pr.d_frame_n, num_frames);
+            pr.values.assign(num_frames, 0.0f);
+            pr.data.dim[0] = (int32_t)num_frames; pr.data.dim[1] = 1; pr.data.dim[2] = 0; pr.data.dim[3] = 0;
+            break;
         case MDGPU_OP_RMSD: {   // an empty selection is valid and evaluates to 0 (_rmsd :4311, :4336-4338)
             std::vector<int2> pairs;   // without bonds md_util_unwrap_vec4 fails and its result is ignored (:4327): nothing is unwrapped
             build_unwrap_pairs(pairs, pr.h_idx[0].size(), p->conn_off, p->conn_idx);
@@ -693,6 +712,10 @@ mdgpu_plan* mdgpu_plan_create(const mdgpu_system_desc_t* sys, const mdgpu_proper
             p->num_atoms_c = p->needed.size(); p->axis_stride_c = (p->num_atoms_c + 3) & ~(size_t)3;
             std::vector<float> mc(p->num_atoms_c); for (size_t j = 0; j < mc.size(); ++j) mc[j] = p->h_mass[(size_t)p->needed[j]];
             if (upload(&p->d_mass_c, mc.data(), mc.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (masses)");
+            if (!p->h_radius.empty()) {
+                std::vector<float> rc(p->num_atoms_c); for (size_t j = 0; j < rc.size(); ++j) rc[j] = p->h_radius[(size_t)p->needed[j]];
+                if (upload(&p->d_radius_c, rc.data(), rc.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (radii)");
+            }
             for (auto& pr : p->props) for (int k = 0; k < 4; ++k) if (!pr.h_idx[k].empty()) {
                 std::vector<int32_t> ci(pr.h_idx[k].size()); for (size_t j = 0; j < ci.size(); ++j) ci[j] = pr.h_idx[k][j] < 0 ? -1 : map[(size_t)pr.h_idx[k][j]];
                 pr.first_c[k] = ci[0];
@@ -719,6 +742,7 @@ int mdgpu_plan_clear(mdgpu_plan* p) {
         if (pr.d_acc) CUDA_TRY(cudaMemset(pr.d_acc, 0, sizeof(unsigned long long) * MDGPU_DIST_BINS));
         if (pr.d_vol) CUDA_TRY(cudaMemset(pr.d_vol, 0, sizeof(uint32_t) * MDGPU_VOL_DIM * MDGPU_VOL_DIM * MDGPU_VOL_DIM));
         if (pr.d_frame_total) CUDA_TRY(cudaMemset(pr.d_frame_total, 0, sizeof(unsigned long long) * p->num_frames));
+        if (pr.d_frame_n) CUDA_TRY(cudaMemset(pr.d_frame_n, 0, sizeof(unsigned long long) * p->num_frames));
         if (pr.d_frame_min) CUDA_TRY(cudaMemset(pr.d_frame_min, 0, sizeof(uint32_t) * p->num_frames));
         if (pr.d_frame_max) CUDA_TRY(cudaMemset(pr.d_frame_max, 0, sizeof(uint32_t) * p->num_frames));
         if (pr.d_frame_min64) CUDA_TRY(cudaMemset(pr.d_frame_min64, 0, sizeof(unsigned long long) * p->num_frames));
@@ -849,6 +873,11 @@ static int ensure_slots(mdgpu_plan* p, const mdgpu_unitcell_t* first_cell, bool 
                     int rc = alloc_cell_list(ps.trg, p->B, (uint32_t)p->num_atoms, cap); if (rc) return rc;
                     rc = alloc_cell_list(ps.ref, p->B, (uint32_t)std::max<size_t>(pr.h_idx[0].size(), 1), cap); if (rc) return rc;
                     CUDA_TRY(dalloc(&ps.d_flags, (size_t)p->B * p->num_atoms));
+                } else if (pr.op == MDGPU_OP_POROSITY) {
+                    CUDA_TRY(dalloc(&ps.d_poro_xyzr, (size_t)PORO_FRAMES * pr.h_idx[0].size())); CUDA_TRY(dalloc(&ps.d_poro_hdr, PORO_FRAMES));
+                    CUDA_TRY(dalloc(&ps.d_poro_grid, (size_t)PORO_FRAMES * PORO_GRID_WORDS)); CUDA_TRY(dalloc(&ps.d_poro_count, PORO_FRAMES));
+                    CUDA_TRY(cudaMemset(ps.d_poro_grid, 0, sizeof(unsigned long long) * PORO_FRAMES * PORO_GRID_WORDS));
+                    CUDA_TRY(cudaMemset(ps.d_poro_count, 0, sizeof(unsigned long long) * PORO_FRAMES));
                 } else if (pr.op == MDGPU_OP_RMSD) {
                     CUDA_TRY(dalloc(&ps.d_sdf_xyzw, (size_t)p->B * 2 * pr.h_idx[0].size()));   // [B][initial, current][atoms]
                 } else if (pr.op == MDGPU_OP_PLANE || pr.op == MDGPU_OP_SHAPE_WEIGHTS) {
@@ -1057,6 +1086,17 @@ static int enqueue_batch(mdgpu_plan* p, Slot& s, const BatchFrames& fr, uint32_t
             }
             launch_distance_pair(fr, s.d_cells, didx[0], cnt[0], didx[1], cnt[1], ps.d_gpos[0], ps.d_gpos[1], pr.d_temporal, frame0, s.stream);
             break; }
+        case MDGPU_OP_POROSITY:   // sub-batches of PORO_FRAMES frames through the slot's grids
+            for (uint32_t f0 = 0; f0 < (uint32_t)B; f0 += PORO_FRAMES) {
+                const uint32_t nf = std::min<uint32_t>(PORO_FRAMES, (uint32_t)B - f0);
+                PorosityArgs a{};
+                a.frames = BatchFrames{ fr.xyz + (size_t)f0 * fr.frame_stride, fr.frame_stride, fr.axis_stride, nf }; a.cells = s.d_cells + f0;
+                a.idx = didx[0]; a.n = (uint32_t)pr.h_idx[0].size(); a.radius = c ? p->d_radius_c : p->d_radius;
+                a.xyzr = ps.d_poro_xyzr; a.hdr = ps.d_poro_hdr; a.grid = ps.d_poro_grid; a.count = ps.d_poro_count;
+                a.frame_set = pr.d_frame_total; a.frame_n = pr.d_frame_n; a.out = pr.d_temporal; a.frame0 = frame0 + f0;
+                launch_porosity(a, (int)nf, s.stream);
+            }
+            break;
         case MDGPU_OP_RMSD: {
             if (!p->have_init) return fail(MDGPU_ERR_INVALID_ARG, "rmsd '%s' needs the initial frame (mdgpu_plan_set_initial_frame)", pr.name.c_str());
             RmsdArgs a{};
@@ -1265,6 +1305,7 @@ static int multi_sync(mdgpu_plan* p) {
         NCCL_TRY(m, reduce(&Prop::d_acc, MDGPU_DIST_BINS, NCCL_UINT64));
         NCCL_TRY(m, reduce(&Prop::d_vol, NV, NCCL_UINT32));
         NCCL_TRY(m, reduce(&Prop::d_frame_total, F, NCCL_UINT64));
+        NCCL_TRY(m, reduce(&Prop::d_frame_n, F, NCCL_UINT64));
         NCCL_TRY(m, reduce(&Prop::d_frame_min, F, NCCL_UINT32));   // rows of frames a device did not evaluate are zero: the sum merges them
         NCCL_TRY(m, reduce(&Prop::d_frame_max, F, NCCL_UINT32));
         NCCL_TRY(m, reduce(&Prop::d_frame_min64, F, NCCL_UINT64));
@@ -1283,6 +1324,7 @@ static int multi_sync(mdgpu_plan* p) {
             if (pr.d_acc) CUDA_TRY(cudaMemset(pr.d_acc, 0, sizeof(unsigned long long) * MDGPU_DIST_BINS));
             if (pr.d_vol) CUDA_TRY(cudaMemset(pr.d_vol, 0, sizeof(uint32_t) * NV));
             if (pr.d_frame_total) CUDA_TRY(cudaMemset(pr.d_frame_total, 0, sizeof(unsigned long long) * F));
+            if (pr.d_frame_n) CUDA_TRY(cudaMemset(pr.d_frame_n, 0, sizeof(unsigned long long) * F));
             if (pr.d_frame_min) CUDA_TRY(cudaMemset(pr.d_frame_min, 0, sizeof(uint32_t) * F));
             if (pr.d_frame_max) CUDA_TRY(cudaMemset(pr.d_frame_max, 0, sizeof(uint32_t) * F));
             if (pr.d_frame_min64) CUDA_TRY(cudaMemset(pr.d_frame_min64, 0, sizeof(unsigned long long) * F));
@@ -1667,6 +1709,7 @@ static void fold_temporal_rows(Prop& pr, uint32_t f, bool reset) {
 }
 static void temporal_ranges(Prop& pr) {
     if (pr.op == MDGPU_OP_DISTANCE || pr.op == MDGPU_OP_DISTANCE_MIN || pr.op == MDGPU_OP_DISTANCE_MAX || pr.op == MDGPU_OP_DISTANCE_PAIR) { pr.data.min_range[0] = 0.0f; pr.data.max_range[0] = pr.data.max_value; }   // value_range {0, FLT_MAX} (:3884)
+    else if (pr.op == MDGPU_OP_POROSITY) { pr.data.min_range[0] = 0.0f; pr.data.max_range[0] = 1.0f; }   // value_range {0, 1} (:5866)
     else { pr.data.min_range[0] = pr.data.min_value; pr.data.max_range[0] = pr.data.max_value; }
 }
 
@@ -2011,6 +2054,7 @@ int mdgpu_plan_property_frame_rows(mdgpu_plan* p, size_t prop, uint32_t which, v
     Prop& pr = p->props[prop]; const size_t F = p->num_frames;
     *d_ptr = nullptr; *bytes = 0; *elem_bytes = 0;
     if (which == 0 && pr.d_frame_total) { *d_ptr = pr.d_frame_total; *elem_bytes = 8; }
+    else if (which == 1 && pr.d_frame_n) { *d_ptr = pr.d_frame_n; *elem_bytes = 8; }
     else if (which == 1 && pr.d_frame_min) { *d_ptr = pr.d_frame_min; *elem_bytes = 4; }
     else if (which == 1 && pr.d_frame_min64) { *d_ptr = pr.d_frame_min64; *elem_bytes = 8; }
     else if (which == 2 && pr.d_frame_max) { *d_ptr = pr.d_frame_max; *elem_bytes = 4; }

@@ -8,6 +8,7 @@ descriptors. This module exists so that the tests and bench.py can be written th
 Supported statements:  ident = proc(args);   with proc in
     rdf(sel, sel, cutoff | min:max)   sdf(residue(a:b) | sel-array, sel, cutoff)   density_x|_y|_z(sel)
     distance(i, j)   angle(i, j, k)   dihedral(i, j, k, l)            (1-based atom indices as in md_script)
+    porosity(sel)                                                        (needs System.radius)
 Selections (evaluated once, statically, to ascending atom index lists — md_script.c:5492-5524):
     all | element('O') | name('C2*') | resname('SOL') | atom(a:b) | residue(a:b) | `and` / `or` / `not` of these
 `residue(a:b)` used as the first argument of sdf() yields one structure per residue (bitfield array semantics).
@@ -305,6 +306,9 @@ class _Parser:
             p = api.plane(ident, self.groups_or_selection())   # an array of selections: the plane through their centres of mass
         elif proc == "rmsd":
             p = api.rmsd(ident, self.selection())   # an array of selections is flattened into their union (_internal_flatten_bf :4305)
+        elif proc == "porosity":   # an array of selections is flattened into their union (:5888-5891); within() is not lowered here
+            if self._has_within_before_comma(): raise ScriptError("porosity() of a dynamic selection is not lowered")
+            p = api.porosity(ident, self.selection())
         elif proc == "distance":
             a = self.index(True); self.expect("ch", ","); b = self.index(True); p = api.distance(ident, a, b)
         elif proc == "angle":
