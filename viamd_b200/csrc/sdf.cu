@@ -10,8 +10,6 @@
 #include "common.cuh"
 #include "kernels.h"
 #include "pbcmath.cuh"
-#include <string.h>
-#include <stdlib.h>
 
 namespace mdg {
 
@@ -345,9 +343,9 @@ MDG_D int isign(int v) { return (v > 0) - (v < 0); }
 //  * each HALF-warp then walks one cell at a time, 16 points per step (a cell of the bench workload holds ~45 targets: three steps at 94 %
 //    lane use, where a full warp per cell would run two steps at 70 % and a flattened index space pays a boundary search per step);
 //  * the box test passes ~60 % of the candidates (the box is 20 A wide, the 2-3 cells per axis it overlaps 22-33 A), so the transform
-//    and the voxel increment run in place under the hit predicate — compacting hits first costs more than the idle lanes it would fill
-//    (the ring version below spends much of its instructions on the compaction and on set-up).
+//    and the voxel increment run in place under the hit predicate — compacting hits first costs more than the idle lanes it would fill.
 constexpr int SDF_WARPS = 8;
+constexpr int SDF_MIN_CTAS = 4;   // resident CTAs / SM the register allocation of k_sdf_scatter aims for (MINB)
 constexpr int SDF_MAXSEG = 128;
 constexpr int SDF_EXCL_CACHE = 64;
 
@@ -477,131 +475,6 @@ __global__ void __launch_bounds__(SDF_WARPS * 32, MINB) k_sdf_scatter(SdfArgs a,
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) local += __shfl_xor_sync(0xffffffffu, local, o);
     if (lane == 0 && local) atomicAdd(&a.frame_total[a.frame0 + f], (unsigned long long)local);
-}
-
-// The round-1 form: flattened candidate index space (boundary search per step) and a per-warp ring that compacts hits before the splat.
-// Kept selectable (MDGPU_SDF=ring) as the alternative to the half-warp form above.
-constexpr int SDF_RING = 64;
-template <bool TRI>
-__global__ void __launch_bounds__(SDF_WARPS * 32) k_sdf_scatter_ring(SdfArgs a, int B) {
-    const int f = blockIdx.y;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const uint32_t s = blockIdx.x * SDF_WARPS + warp;
-    __shared__ uint32_t s_pre[SDF_WARPS][SDF_MAXSEG + 1];
-    __shared__ uint2 s_seg[SDF_WARPS][SDF_MAXSEG];        // x: start - pre (first point of the segment minus its flattened offset), y: image code
-    __shared__ float s_ring[SDF_WARPS][3][SDF_RING];
-    __shared__ int32_t s_excl[SDF_WARPS][SDF_EXCL_CACHE];
-    if (s >= a.n_struct) return;
-    const FrameGeom& g = a.geom[f];
-    if (g.valid == -1) return;
-    const float* rec = a.matrices + ((size_t)f * a.n_struct + s) * SDF_REC;
-    SdfXform X;
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 3; ++j) X.M[i][j] = rec[i * 4 + j];
-    X.A00 = g.A[0][0]; X.A11 = g.A[1][1]; X.A22 = g.A[2][2]; X.O0 = g.origin[0]; X.O1 = g.origin[1]; X.O2 = g.origin[2];
-    X.A10 = g.A[1][0]; X.A20 = g.A[2][0]; X.A21 = g.A[2][1];
-    const float lo3[3] = { rec[20], rec[21], rec[22] }, hi3[3] = { rec[23], rec[24], rec[25] };
-    const int* ri = (const int*)(rec + 26);
-    const int cmin[3] = { ri[0], ri[1], ri[2] }, cmax[3] = { ri[3], ri[4], ri[5] };
-    const int pbc[3] = { (g.flags & MDGPU_CELL_PBC_X) != 0, (g.flags & MDGPU_CELL_PBC_Y) != 0, (g.flags & MDGPU_CELL_PBC_Z) != 0 };
-    const int cd[3] = { g.cdim[0], g.cdim[1], g.cdim[2] };
-    const float4* __restrict__ pts = a.trg.sorted + (size_t)f * a.trg.max_points;
-    const uint32_t* __restrict__ off = a.trg.cell_cnt + (size_t)f * (a.trg.cap + 1);
-    const int32_t* sidx = a.struct_idx + (size_t)s * a.struct_size;
-    // exclusion mask = the structure's own atoms (:5674). Ascending index lists: a contiguous run (the usual case: a residue)
-    // is tested with one compare; otherwise the list (cached in shared memory when it fits) is scanned.
-    const uint32_t ex_lo = (uint32_t)sidx[0], ex_n = a.struct_size;
-    const bool ex_contig = ((uint32_t)sidx[a.struct_size - 1] - ex_lo + 1u) == ex_n;
-    if (!ex_contig) { for (uint32_t k = lane; k < min(ex_n, (uint32_t)SDF_EXCL_CACHE); k += 32) s_excl[warp][k] = sidx[k]; }
-    const int ex = cmax[0] - cmin[0], ey = cmax[1] - cmin[1], ez = cmax[2] - cmin[2];
-    const int ncells = ex * ey * ez;
-    const uint32_t lt = (1u << lane) - 1u;
-    float* rx = s_ring[warp][0]; float* ry = s_ring[warp][1]; float* rz = s_ring[warp][2];
-    uint32_t cnt = 0;                      // candidates waiting in the ring (warp-uniform, < 32 between steps)
-    unsigned long long local = 0;
-    for (int c0 = 0; c0 < ncells; c0 += SDF_MAXSEG) {   // (:1925-1943) cells of the range, SDF_MAXSEG at a time
-        const int nc = min(SDF_MAXSEG, ncells - c0);
-        uint32_t base = 0; int nseg = 0;
-        __syncwarp();
-        for (int n0 = 0; n0 < nc; n0 += 32) {
-            const int n = n0 + lane;
-            uint32_t len = 0, start = 0, code = 0x15;
-            if (n < nc) {
-                const int q = c0 + n;
-                const int icx = cmin[0] + q % ex, icy = cmin[1] + (q / ex) % ey, icz = cmin[2] + q / (ex * ey);
-                const int cx = pbc[0] ? wrap_coord(icx, cd[0]) : icx, cy = pbc[1] ? wrap_coord(icy, cd[1]) : icy, cz = pbc[2] ? wrap_coord(icz, cd[2]) : icz;
-                if (!(cx < 0 || cx >= cd[0] || cy < 0 || cy >= cd[1] || cz < 0 || cz >= cd[2])) {
-                    const uint32_t ci = ((uint32_t)cz * (uint32_t)cd[1] + (uint32_t)cy) * (uint32_t)cd[0] + (uint32_t)cx;
-                    start = off[ci]; len = off[ci + 1] - start;
-                    code = (uint32_t)(isign(icx - cx) + 1) | ((uint32_t)(isign(icy - cy) + 1) << 2) | ((uint32_t)(isign(icz - cz) + 1) << 4);
-                }
-            }
-            const uint32_t have = __ballot_sync(0xffffffffu, len != 0u);   // keep non-empty cells only
-            uint32_t incl = len;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
-            if (len) { const int slot = nseg + __popc(have & lt); const uint32_t pre = base + incl - len; s_pre[warp][slot] = pre; s_seg[warp][slot] = make_uint2(start - pre, code); }
-            base += __shfl_sync(0xffffffffu, incl, 31);
-            nseg += __popc(have);
-        }
-        const uint32_t total = base;
-        if (lane == 0) s_pre[warp][nseg] = total;
-        __syncwarp();
-        int kbase = 0;                     // segment that contains candidate j0 (warp-uniform)
-        for (uint32_t j0 = 0; j0 < total; j0 += 32) {
-            // segment boundaries inside (j0, j0+32]: bit (b - j0 - 1). Segments are non-empty, so they are among the next 32 table entries.
-            const int kb = kbase + 1 + lane;
-            const uint32_t bnd = (kb <= nseg) ? s_pre[warp][kb] : 0xffffffffu;
-            const uint32_t rel = bnd - j0 - 1u;
-            const uint32_t bm = __reduce_or_sync(0xffffffffu, rel < 32u ? (1u << rel) : 0u);
-            const uint32_t j = j0 + lane;
-            bool hit = false; float vx = 0.f, vy = 0.f, vz = 0.f;
-            if (j < total) {
-                const uint2 sg = s_seg[warp][kbase + __popc(bm & lt)];
-                const float4 t = pts[sg.x + j];
-                vx = t.x; vy = t.y; vz = t.z;
-                if (sg.y != 0x15u) {   // periodic image of the cell: + (-1|0|+1), rounded (:1962-1964); +0 is the identity
-                    vx = __fadd_rn(vx, (float)((int)(sg.y & 3u) - 1)); vy = __fadd_rn(vy, (float)((int)((sg.y >> 2) & 3u) - 1)); vz = __fadd_rn(vz, (float)((int)((sg.y >> 4) & 3u) - 1));
-                }
-                if (TRI) {   // box test on the cartesian image (fract_to_cart_tri_256 md_spatial_acc.c:594-603), all axes periodic (:2009)
-                    const float cx_ = __fmaf_rn(vx, X.A00, __fmaf_rn(vy, X.A10, __fmaf_rn(vz, X.A20, X.O0))), cy_ = __fmaf_rn(vy, X.A11, __fmaf_rn(vz, X.A21, X.O1)), cz_ = __fmaf_rn(vz, X.A22, X.O2);
-                    hit = cx_ >= lo3[0] && cy_ >= lo3[1] && cz_ >= lo3[2] && cx_ <= hi3[0] && cy_ <= hi3[1] && cz_ <= hi3[2];
-                } else hit = vx >= lo3[0] && vy >= lo3[1] && vz >= lo3[2] && vx <= hi3[0] && vy <= hi3[1] && vz <= hi3[2];
-                if (hit) {
-                    const uint32_t idx = __float_as_uint(t.w);
-                    if (ex_contig) hit = (idx - ex_lo) >= ex_n;
-                    else {
-                        bool excluded = false;
-                        const uint32_t nc_ = min(ex_n, (uint32_t)SDF_EXCL_CACHE);
-                        for (uint32_t q = 0; q < nc_; ++q) excluded |= ((uint32_t)s_excl[warp][q] == idx);
-                        for (uint32_t q = nc_; q < ex_n; ++q) excluded |= ((uint32_t)sidx[q] == idx);
-                        hit = !excluded;
-                    }
-                }
-            }
-            kbase += __popc(bm);
-            const uint32_t hm = __ballot_sync(0xffffffffu, hit);
-            if (hit) { const uint32_t p = cnt + __popc(hm & lt); rx[p] = vx; ry[p] = vy; rz[p] = vz; }
-            cnt += __popc(hm);
-            if (cnt >= 32u) {
-                __syncwarp();
-                sdf_splat<TRI>(rx[lane], ry[lane], rz[lane], X, a.vol);
-                const uint32_t rem = cnt - 32u;
-                float mx = 0.f, my = 0.f, mz = 0.f;
-                if (lane < rem) { mx = rx[32 + lane]; my = ry[32 + lane]; mz = rz[32 + lane]; }
-                __syncwarp();
-                if (lane < rem) { rx[lane] = mx; ry[lane] = my; rz[lane] = mz; }
-                cnt = rem; local += 32;
-                __syncwarp();
-            }
-        }
-    }
-    __syncwarp();
-    if (lane < cnt) sdf_splat<TRI>(rx[lane], ry[lane], rz[lane], X, a.vol);
-    local += cnt;
-    if (lane == 0 && local) atomicAdd(&a.frame_total[a.frame0 + f], local);
 }
 
 // ------------------------------------------------------------------------------------------------- rmsd(selection)
@@ -851,14 +724,7 @@ void launch_sdf(const SdfArgs& a, int B, bool tri, cudaStream_t s) {
     k_sdf_fit<<<g1, 64, 0, s>>>(a, B);
     note_launch("k_sdf_fit", s);
     dim3 g2((a.n_struct + SDF_WARPS - 1) / SDF_WARPS, B);
-    static const bool ring = []() { const char* e = getenv("MDGPU_SDF"); return e && strcmp(e, "ring") == 0; }();
-    if (ring) { if (tri) k_sdf_scatter_ring<true><<<g2, SDF_WARPS * 32, 0, s>>>(a, B); else k_sdf_scatter_ring<false><<<g2, SDF_WARPS * 32, 0, s>>>(a, B); }
-    else {
-        static const int occ = []() { const char* e = getenv("MDGPU_SDF_OCC"); return e ? atoi(e) : 4; }();   // resident CTAs / SM the register allocation aims for
-        if (occ >= 5)      { if (tri) k_sdf_scatter<true, 5><<<g2, SDF_WARPS * 32, 0, s>>>(a, B); else k_sdf_scatter<false, 5><<<g2, SDF_WARPS * 32, 0, s>>>(a, B); }
-        else if (occ == 4) { if (tri) k_sdf_scatter<true, 4><<<g2, SDF_WARPS * 32, 0, s>>>(a, B); else k_sdf_scatter<false, 4><<<g2, SDF_WARPS * 32, 0, s>>>(a, B); }
-        else               { if (tri) k_sdf_scatter<true, 3><<<g2, SDF_WARPS * 32, 0, s>>>(a, B); else k_sdf_scatter<false, 3><<<g2, SDF_WARPS * 32, 0, s>>>(a, B); }
-    }
+    if (tri) k_sdf_scatter<true, SDF_MIN_CTAS><<<g2, SDF_WARPS * 32, 0, s>>>(a, B); else k_sdf_scatter<false, SDF_MIN_CTAS><<<g2, SDF_WARPS * 32, 0, s>>>(a, B);
     note_launch("k_sdf_scatter", s);
 }
 
