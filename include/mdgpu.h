@@ -387,6 +387,12 @@ int mdgpu_debug_aggregate(const float* values, size_t count, float* out4);
  * float whose bit pattern lies in [lo_bits, hi_bits) and returns the number of mismatches (must be 0 in the normal range). */
 int mdgpu_debug_sqrt_sweep(int device, uint32_t lo_bits, uint32_t hi_bits, uint64_t* mismatches);
 
+/* The rdf candidate cull this process runs (no device needed): "full8" / "full6" / "full4" (full-warp cull at that register target, the
+ * default is full8), "half" (half-warp cull) or "flat6" / "flat8" / "flat4" (flattened cull). MDGPU_CULL and MDGPU_CULL_OCC are read once, at
+ * the first rdf launch or the first call of this function, whichever comes first; later changes of the environment have no effect.
+ * Writes a NUL-terminated name into out[n]. */
+int mdgpu_debug_rdf_config(char* out, size_t n);
+
 /* Synthetic workloads (viamd_b200/csrc/synth.h), used by bench.py and the tests. */
 int mdgpu_synth_water_desc(uint32_t n, uint32_t seed, uint32_t* num_atoms, float* L);
 int mdgpu_synth_water_base(uint32_t n, uint32_t seed, float* base_xyz /* [3][num_atoms] wrapped */, float* whole_xyz /* optional */);

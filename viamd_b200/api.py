@@ -899,6 +899,14 @@ def debug_sqrt_sweep(lo_bits: int, hi_bits: int, device: int = 0) -> int:
     return int(n.value)
 
 
+def debug_rdf_config() -> str:
+    """the rdf candidate cull of this process (mdgpu_debug_rdf_config): full8 | full6 | full4 | half | flat6 | flat8 | flat4"""
+    buf = C.create_string_buffer(16)
+    lib().mdgpu_debug_rdf_config.argtypes = [C.c_char_p, C.c_size_t]
+    _check(lib().mdgpu_debug_rdf_config(buf, len(buf)))
+    return buf.value.decode()
+
+
 def water_system(n: int) -> System:
     """Topology of the synthetic water box (OW,HW1,HW2 per molecule; masses as md_atom_extract_masses yields them)."""
     nm = n ** 3; na = 3 * nm

@@ -40,6 +40,10 @@ struct RdfArgs {
 };
 void launch_group_com(const BatchFrames& fr, const int32_t* d_idx, const uint32_t* d_off, uint32_t n_groups, const float* d_mass, float* d_out, cudaStream_t s);
 void launch_rdf(const RdfArgs& a, int B, bool tri, int variant, int sm_count, cudaStream_t s, cudaEvent_t* ev4 /* null, or events recorded {before cull, after cull, before pairs, after pairs} */);
+// the candidate cull launch_rdf runs (MDGPU_CULL / MDGPU_CULL_OCC, read once per process)
+enum RdfCullKind { RDF_CULL_FULL = 0, RDF_CULL_HALF = 1, RDF_CULL_FLAT = 2 };
+struct RdfCullConfig { int kind; int occ; };   // occ: resident CTAs / SM the register allocation aims for (8, 6 or 4; 0 for the half-warp cull)
+RdfCullConfig rdf_cull_config();
 
 void launch_contact_rows(const uint32_t* d_frame_bins, uint32_t n_sets, float* d_out, uint32_t frame0, int B, cudaStream_t s);   // running totals over the sets -> temporal row
 unsigned long long run_sqrt_sweep(uint32_t lo_bits, uint32_t hi_bits);

@@ -2143,6 +2143,17 @@ int mdgpu_debug_sqrt_sweep(int device, uint32_t lo_bits, uint32_t hi_bits, uint6
     return 0;
 }
 
+int mdgpu_debug_rdf_config(char* out, size_t n) {
+    if (!out) return fail(MDGPU_ERR_INVALID_ARG, "null argument");
+    const RdfCullConfig c = rdf_cull_config();
+    char name[16];
+    if (c.kind == RDF_CULL_HALF) snprintf(name, sizeof(name), "half");
+    else snprintf(name, sizeof(name), "%s%d", c.kind == RDF_CULL_FLAT ? "flat" : "full", c.occ);
+    if (strlen(name) >= n) return fail(MDGPU_ERR_INVALID_ARG, "mdgpu_debug_rdf_config: buffer of %zu bytes too small", n);
+    memcpy(out, name, strlen(name) + 1);
+    return 0;
+}
+
 // ------------------------------------------------------------------------------------------------- synthetic workloads
 int mdgpu_synth_water_desc(uint32_t n, uint32_t seed, uint32_t* num_atoms, float* L) {
     const mdsynth_water_t w = mdsynth_water_desc(n, seed);
