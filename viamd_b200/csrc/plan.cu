@@ -18,6 +18,8 @@
 #include <chrono>
 #include <string>
 #include <thread>
+#include <type_traits>
+#include <utility>
 #include <vector>
 #include <map>
 #include <algorithm>
@@ -40,42 +42,96 @@ static int fail(int code, const char* fmt, ...) {
 
 void note_launch(const char*, cudaStream_t) { g_launches.fetch_add(1, std::memory_order_relaxed); }
 
-template <typename T> static cudaError_t dalloc(T** p, size_t n) { *p = nullptr; return n ? cudaMalloc((void**)p, n * sizeof(T)) : cudaSuccess; }
-template <typename T> static cudaError_t upload(T** p, const T* h, size_t n) {
-    cudaError_t e = dalloc(p, n); if (e != cudaSuccess || !n) return e;
-    return cudaMemcpy(*p, h, n * sizeof(T), cudaMemcpyHostToDevice);
-}
+// Owner of one allocation of n elements of T, in device memory or (Host) pinned host memory: freed when the owner is destroyed or
+// reallocated, so a buffer's lifetime is its owner's and a failed allocation leaves an empty owner. Move-only.
+template <typename T, bool Host = false> class Buf {
+    T* p_ = nullptr; size_t n_ = 0;
+public:
+    using value_type = T;
+    Buf() = default;
+    Buf(const Buf&) = delete; Buf& operator=(const Buf&) = delete;
+    Buf(Buf&& o) noexcept { *this = std::move(o); }
+    Buf& operator=(Buf&& o) noexcept { std::swap(p_, o.p_); std::swap(n_, o.n_); return *this; }   // o frees what this held
+    ~Buf() { reset(); }
+    void reset() { if (p_) { if (Host) cudaFreeHost(p_); else cudaFree(p_); } p_ = nullptr; n_ = 0; }
+    cudaError_t alloc(size_t n) {   // n == 0 allocates nothing
+        reset();
+        if (!n) return cudaSuccess;
+        void* q = nullptr; const cudaError_t e = Host ? cudaMallocHost(&q, n * sizeof(T)) : cudaMalloc(&q, n * sizeof(T));
+        if (e == cudaSuccess) { p_ = (T*)q; n_ = n; }
+        return e;
+    }
+    cudaError_t upload(const T* h, size_t n) {
+        static_assert(!Host, "pinned buffers are written directly");
+        const cudaError_t e = alloc(n); if (e != cudaSuccess || !n) return e;
+        return cudaMemcpy(p_, h, n * sizeof(T), cudaMemcpyHostToDevice);
+    }
+    T* get() const { return p_; }
+    size_t size() const { return n_; }
+    size_t bytes() const { return n_ * sizeof(T); }
+    T& operator[](size_t i) const { static_assert(Host, "device memory is not addressable from the host"); return p_[i]; }
+};
+template <typename T> using DevBuf = Buf<T, false>;
+template <typename T> using PinnedBuf = Buf<T, true>;
+
+// Owner of a stream or event, destroyed with its owner; it converts to the handle for the runtime calls that use it.
+template <typename H, cudaError_t (*Destroy)(H)> class Handle {
+    H h_ = nullptr;
+public:
+    Handle() = default;
+    Handle(const Handle&) = delete; Handle& operator=(const Handle&) = delete;
+    Handle(Handle&& o) noexcept { std::swap(h_, o.h_); }
+    Handle& operator=(Handle&& o) noexcept { std::swap(h_, o.h_); return *this; }
+    ~Handle() { if (h_) Destroy(h_); }
+    H* out() { if (h_) Destroy(h_); h_ = nullptr; return &h_; }   // where a create call writes the new handle
+    operator H() const { return h_; }
+};
+using Stream = Handle<cudaStream_t, cudaStreamDestroy>;
+using Event = Handle<cudaEvent_t, cudaEventDestroy>;
+
+// Owner of the arrays of one CellList; `cl` is the plain struct the kernels receive (empty until alloc succeeds).
+struct CellListBuf {
+    DevBuf<float4> sorted, scratch; DevBuf<uint32_t> cell_of, rank, cell_cnt;
+    CellList cl{};
+    cudaError_t alloc(uint32_t B, uint32_t max_points, uint32_t cap) {
+        const size_t n = (size_t)B * max_points; cudaError_t e;
+        if ((e = sorted.alloc(n)) != cudaSuccess || (e = scratch.alloc(n)) != cudaSuccess || (e = cell_of.alloc(n)) != cudaSuccess ||
+            (e = rank.alloc(n)) != cudaSuccess || (e = cell_cnt.alloc((size_t)B * (cap + 1) + B)) != cudaSuccess) return e;
+        cl = CellList{ sorted.get(), scratch.get(), cell_of.get(), rank.get(), cell_cnt.get(), cell_cnt.get() + (size_t)B * (cap + 1), max_points, cap };
+        return cudaSuccess;
+    }
+};
 
 struct Prop {
     std::string name; uint32_t op = 0;
-    std::vector<int32_t> h_idx[4]; int32_t* d_idx[4] = { nullptr, nullptr, nullptr, nullptr };
-    int32_t* d_idx_c[4] = { nullptr, nullptr, nullptr, nullptr };   // the same lists in the plan's compact atom space (host ingest of selected atoms)
-    int32_t first_c[4] = { 0, 0, 0, 0 };                            // compact index of each list's first atom (single-atom arguments are passed by value)
+    std::vector<int32_t> h_idx[4]; DevBuf<int32_t> d_idx[4];
+    DevBuf<int32_t> d_idx_c[4];                    // the same lists in the plan's compact atom space (host ingest of selected atoms)
+    int32_t first_c[4] = { 0, 0, 0, 0 };           // compact index of each list's first atom (single-atom arguments are passed by value)
     size_t n_struct = 0, struct_size = 0;
     uint32_t com_mask = 0;   // distance/angle/dihedral: bit k = argument k is a selection evaluated through md_util_com_compute
-    std::vector<uint32_t> h_soff; uint32_t* d_soff = nullptr;   // rdf with centre-of-mass references: CSR offsets of the groups in idx[0]
+    std::vector<uint32_t> h_soff; DevBuf<uint32_t> d_soff;   // rdf with centre-of-mass references: CSR offsets of the groups in idx[0]
     float cutoff_min = 0.f, cutoff_max = 0.f;
-    std::vector<uint32_t> h_goff[2]; uint32_t* d_goff[2] = { nullptr, nullptr };   // distance_pair: CSR groups of argument 0 / 1 (arrays of selections)
-    std::vector<uint32_t> h_aoff[4]; uint32_t* d_aoff[4] = { nullptr, nullptr, nullptr, nullptr };   // distance / angle / dihedral / com: argument k is an ARRAY of selections (centre of their centres)
-    uint8_t* d_and_mask = nullptr;   // `selection and within(...)`: one byte per atom of the static side (count(within()) / rdf(within()))
+    std::vector<uint32_t> h_goff[2]; DevBuf<uint32_t> d_goff[2];   // distance_pair: CSR groups of argument 0 / 1 (arrays of selections)
+    std::vector<uint32_t> h_aoff[4]; DevBuf<uint32_t> d_aoff[4];   // distance / angle / dihedral / com: argument k is an ARRAY of selections (centre of their centres)
+    DevBuf<uint8_t> d_and_mask;   // `selection and within(...)`: one byte per atom of the static side (count(within()) / rdf(within()))
     float ref_within = 0.f, ref_within_min = 0.f;   // (kept for messages) rdf reference given through the round-1 fields; folded into dyn[0]
     // Dynamic arguments: argument k is within([rmin:]rmax, h_idx[k]) [and a static selection], evaluated per frame on the device into an ascending
     // index list (md_script_functions.inl:2485-2720); the consumers read that list instead of the static one.
-    struct DynArg { bool on = false; float rmin = 0.f, rmax = 0.f; uint8_t* d_and_mask = nullptr; } dyn[4];
+    struct DynArg { bool on = false; float rmin = 0.f, rmax = 0.f; DevBuf<uint8_t> d_and_mask; } dyn[4];
     bool any_dyn() const { return dyn[0].on || dyn[1].on || dyn[2].on || dyn[3].on; }
-    // device accumulators
-    unsigned long long* d_acc = nullptr;          // rdf: 1024 bins; density: 1024 fixed-point sums
-    uint32_t* d_vol = nullptr;                    // sdf: 128^3
-    float* d_vol_mean = nullptr; bool values_registered = false;   // sdf: device-side fold target; host values pinned for the D2H
-    unsigned long long* d_frame_total = nullptr;  // rdf / sdf: [num_frames]
-    uint32_t* d_frame_min = nullptr; uint32_t* d_frame_max = nullptr;             // rdf
-    unsigned long long* d_frame_min64 = nullptr; unsigned long long* d_frame_max64 = nullptr;   // density
-    uint32_t* d_keep = nullptr; unsigned long long* d_keep64 = nullptr;
-    float* d_temporal = nullptr;                  // [num_frames][len]
+    // device accumulators (the result accumulators are listed once, in for_each_accumulator)
+    DevBuf<unsigned long long> d_acc;             // rdf: 1024 bins; density: 1024 fixed-point sums
+    DevBuf<uint32_t> d_vol;                       // sdf: 128^3
+    DevBuf<float> d_vol_mean; bool values_registered = false;   // sdf: device-side fold target; host values pinned for the D2H
+    DevBuf<unsigned long long> d_frame_total;     // rdf / sdf: [num_frames]
+    DevBuf<uint32_t> d_frame_min, d_frame_max;                     // rdf
+    DevBuf<unsigned long long> d_frame_min64, d_frame_max64;       // density
+    DevBuf<uint32_t> d_keep; DevBuf<unsigned long long> d_keep64;
+    DevBuf<float> d_temporal;                     // [num_frames][len]
     size_t len = 1;                               // values per frame of a temporal (distance_pair: |a| * |b|)
     std::vector<float> agg_mean, agg_var, agg_ext;   // len > 1: per-frame mean / population variance / (min, max) (md_script_aggregate_t)
     // sdf statics
-    int2* d_unwrap = nullptr; uint32_t n_unwrap = 0;
+    DevBuf<int2> d_unwrap; uint32_t n_unwrap = 0;
     // density statics (from the initial frame's cell)
     float rc = 0, re = 0, inv_ext = 0, min_point = 0; double dens_factor = 0;
     // results: `values` is the default storage; mdgpu_plan_bind_property_storage points vptr (and the aggregate rows) at the caller's arrays
@@ -86,41 +142,52 @@ struct Prop {
     bool frames_overridden = false;
     bool is_dist() const { return op == MDGPU_OP_RDF || (op >= MDGPU_OP_DENSITY_X && op <= MDGPU_OP_DENSITY_Z); }
     bool needs_cells() const { return op == MDGPU_OP_RDF || op == MDGPU_OP_SDF || op == MDGPU_OP_CONTACT_COUNT; }
-    uint32_t* d_set_of = nullptr;   // contact_count: set of every atom of the concatenated A list
+    DevBuf<uint32_t> d_set_of;   // contact_count: set of every atom of the concatenated A list
     int share_trg = -1;   // index of an earlier property with the same target selection and cutoff: its target cell list is reused
     size_t trg_groups = 0;   // rdf: the target argument was an ARRAY of selections: one centre of mass per selection is the target point (h_goff[1] = their CSR offsets in idx[1])
     size_t backbone_segments = 0;   // MDGPU_OP_BACKBONE_ANGLES (evaluated as 2 dihedrals in context per segment): the segments of its (phi, psi) rows
-    unsigned long long* d_frame_n = nullptr;   // porosity: voxels of each frame's grid (N); d_frame_total holds the occupied ones
+    DevBuf<unsigned long long> d_frame_n;   // porosity: voxels of each frame's grid (N); d_frame_total holds the occupied ones
+
+    // The result accumulators, each once: f(&Prop::member) in turn until one returns non-zero. They are zeroed by mdgpu_plan_clear, and
+    // multi_sync sums them onto the root device (rows of frames a device did not evaluate are zero there) and zeroes them on the peers.
+    // An accumulator that is missing here keeps its values across a clear and is never merged.
+    template <typename F> static int for_each_accumulator(F&& f) {
+        int rc = 0;
+        auto one = [&](auto member) { if (!rc) rc = f(member); };
+        one(&Prop::d_acc); one(&Prop::d_vol); one(&Prop::d_frame_total); one(&Prop::d_frame_n); one(&Prop::d_frame_min); one(&Prop::d_frame_max);
+        one(&Prop::d_frame_min64); one(&Prop::d_frame_max64); one(&Prop::d_keep); one(&Prop::d_keep64); one(&Prop::d_temporal);
+        return rc;
+    }
 };
 
 struct PropScratch {   // per (stream slot, property)
-    FrameGeom* d_geom = nullptr; float* d_aabb = nullptr;
-    CellList trg{}, ref{};
-    uint32_t* d_frame_bins = nullptr; unsigned long long* d_frame_bins64 = nullptr;
-    float4* d_sdf_xyzw = nullptr; float* d_sdf_ref0 = nullptr; float* d_sdf_mats = nullptr;
-    float* d_com = nullptr;   // rdf with centre-of-mass references: [B][n_struct][3]
-    float* d_argpos = nullptr;   // distance/angle/dihedral with selection arguments: [B][4][3]
-    float* d_gpos[2] = { nullptr, nullptr };   // distance_pair with arrays of selections: [B][n_groups][3] per argument
-    float4* d_parts[4] = { nullptr, nullptr, nullptr, nullptr };   // array-of-selections arguments: [B][n_parts] centres (xyz, 1)
-    uint8_t* d_flags = nullptr;  // count(within()) / rdf(within(), ...): [B][num_atoms]
+    DevBuf<FrameGeom> d_geom; DevBuf<float> d_aabb;
+    CellListBuf trg, ref;
+    DevBuf<uint32_t> d_frame_bins; DevBuf<unsigned long long> d_frame_bins64;
+    DevBuf<float4> d_sdf_xyzw; DevBuf<float> d_sdf_ref0, d_sdf_mats;
+    DevBuf<float> d_com;       // rdf with centre-of-mass references: [B][n_struct][3]
+    DevBuf<float> d_argpos;    // distance/angle/dihedral with selection arguments: [B][4][3]
+    DevBuf<float> d_gpos[2];   // distance_pair with arrays of selections: [B][n_groups][3] per argument
+    DevBuf<float4> d_parts[4];   // array-of-selections arguments: [B][n_parts] centres (xyz, 1)
+    DevBuf<uint8_t> d_flags;   // count(within()) / rdf(within(), ...): [B][num_atoms]
     // per dynamic argument: the system-wide grid + lists of its within() query (get_spatial_acc :734), the marks and the per-frame index list
-    struct DynScratch { FrameGeom* d_geom = nullptr; float* d_aabb = nullptr; CellList trg{}, ref{}; uint8_t* d_flags = nullptr; int32_t* d_idx = nullptr; uint32_t* d_n = nullptr; } dynw[4];
-    // rdf candidate lists (k_rdf_cull): [B][list_stride] entries, [B][cap] headers, [B] cursors
-    uint32_t* d_pair_list = nullptr; uint4* d_list_hdr = nullptr; uint32_t* d_list_cursor = nullptr; size_t list_stride = 0;
-    mdgpu_unitcell_t nn_cell{}; size_t nn_of_cell = 0; bool nn_valid = false;   // neighbour-offset count of the last cell seen (list sizing)
+    struct DynScratch { DevBuf<FrameGeom> d_geom; DevBuf<float> d_aabb; CellListBuf trg, ref; DevBuf<uint8_t> d_flags; DevBuf<int32_t> d_idx; DevBuf<uint32_t> d_n; } dynw[4];
+    // rdf candidate lists (k_rdf_cull): [B][list stride] entries, [B][cap] headers, [B] cursors
+    DevBuf<uint32_t> d_pair_list; DevBuf<uint4> d_list_hdr; DevBuf<uint32_t> d_list_cursor;
+    mdgpu_unitcell_t nn_cell{}; size_t nn_stride = 0; bool nn_valid = false;   // candidate-list stride of the last cell seen (list sizing)
     // porosity: per sub-batch of PORO_FRAMES frames the spheres, grid headers, bit grids (zero between sub-batches) and occupied-voxel counters
-    float4* d_poro_xyzr = nullptr; PorosityHdr* d_poro_hdr = nullptr; unsigned long long* d_poro_grid = nullptr; unsigned long long* d_poro_count = nullptr;
+    DevBuf<float4> d_poro_xyzr; DevBuf<PorosityHdr> d_poro_hdr; DevBuf<unsigned long long> d_poro_grid, d_poro_count;
 };
 
 struct Slot {
-    cudaStream_t stream = nullptr; cudaEvent_t done = nullptr; bool busy = false;
+    Stream stream; Event done; bool busy = false;
     bool owned = false;                        // a caller thread holds the slot (acquire_slot / release_slot); guarded by mdgpu_plan::slot_mutex
-    cudaEvent_t copied = nullptr;              // recorded after the batch's host->device copy: the caller's source buffer is free again
-    int* h_err = nullptr;                      // pinned mirror of d_err, copied at the end of every batch (read when the slot is retired)
-    float* d_frames = nullptr; float* h_frames = nullptr;      // staging for host-resident frames (ingest atom space)
-    float* d_xtc_frames = nullptr;                             // whole decoded frames (XTC input)
-    mdgpu_unitcell_t* d_cells = nullptr; mdgpu_unitcell_t* h_cells = nullptr;
-    int* d_err = nullptr;
+    Event copied;                              // recorded after the batch's host->device copy: the caller's source buffer is free again
+    PinnedBuf<int> h_err;                      // pinned mirror of d_err, copied at the end of every batch (read when the slot is retired)
+    DevBuf<float> d_frames; PinnedBuf<float> h_frames;   // staging for host-resident frames (ingest atom space)
+    DevBuf<float> d_xtc_frames;                          // whole decoded frames (XTC input)
+    DevBuf<mdgpu_unitcell_t> d_cells; PinnedBuf<mdgpu_unitcell_t> h_cells;
+    DevBuf<int> d_err;
     std::vector<PropScratch> ps;
     uint32_t pending_beg = 0, pending_cnt = 0;
 };
@@ -137,9 +204,9 @@ static uint32_t xtc_super() {   // batches per scan stage; MDGPU_XTC_SUPER overr
 
 constexpr uint32_t XTC_STAGES = 3;   // the scan of super-batch k+2 is in flight while the batches of k are expanded and evaluated
 struct XtcStage {
-    cudaStream_t stream = nullptr; cudaEvent_t ready = nullptr; cudaEvent_t consumed[XTC_SUPER_MAX] = {}; uint32_t n_consumed = 0;
-    uint8_t* d_blob = nullptr; size_t cap = 0; unsigned long long* d_off = nullptr; unsigned long long* h_off = nullptr;
-    XtcFrameInfo* d_info = nullptr; uint2* d_rec = nullptr; uint16_t* d_state = nullptr;
+    Stream stream; Event ready; Event consumed[XTC_SUPER_MAX]; uint32_t n_consumed = 0;
+    DevBuf<uint8_t> d_blob; DevBuf<unsigned long long> d_off; PinnedBuf<unsigned long long> h_off;
+    DevBuf<XtcFrameInfo> d_info; DevBuf<uint2> d_rec; DevBuf<uint16_t> d_state;
 };
 
 struct TimedLaunch { cudaEvent_t a, b; int kind; };   // kind: 0 rdf pair kernel, 1 sdf (all three kernels), 2 density (+finalize), 3 rdf cull kernel
@@ -155,6 +222,10 @@ struct NcclApi {
     const char* (*GetErrorString)(int) = nullptr;
 };
 enum { NCCL_UINT32 = 3, NCCL_UINT64 = 5, NCCL_FLOAT32 = 7, NCCL_SUM = 0 };   // ncclDataType_t / ncclRedOp_t values (nccl.h)
+template <typename T> constexpr int nccl_type() {
+    static_assert(std::is_same<T, uint32_t>::value || std::is_same<T, unsigned long long>::value || std::is_same<T, float>::value, "no NCCL type");
+    return std::is_same<T, uint32_t>::value ? NCCL_UINT32 : std::is_same<T, float>::value ? NCCL_FLOAT32 : NCCL_UINT64;
+}
 
 struct MultiDevice {
     std::vector<mdgpu_plan*> peers;    // devices[1..]; the root plan is devices[0]
@@ -173,16 +244,16 @@ struct mdgpu_plan {
     int device = 0; int sm_count = 132;
     size_t num_atoms = 0, num_frames = 0; size_t axis_stride = 0;   // staging layout: [frame][3][axis_stride]
     uint32_t B = 132; uint32_t S = 2; uint32_t cell_cap = 0; bool keep = false; uint32_t rdf_variant = 0;
-    std::vector<float> h_mass; float* d_mass = nullptr;
-    std::vector<float> h_radius; float* d_radius = nullptr; float* d_radius_c = nullptr;   // van der Waals radii (porosity plans only)
+    std::vector<float> h_mass; DevBuf<float> d_mass;
+    std::vector<float> h_radius; DevBuf<float> d_radius, d_radius_c;   // van der Waals radii (porosity plans only)
     // Compact atom space: the union of the atoms any property reads, ascending. When it is well below the system size, host ingest copies
     // only those atoms (gathered into pinned staging by the ingest threads) and the kernels run on index lists remapped into that space.
-    bool compact = false; std::vector<int32_t> needed; size_t num_atoms_c = 0, axis_stride_c = 0; float* d_mass_c = nullptr; float* d_init_c = nullptr;
+    bool compact = false; std::vector<int32_t> needed; size_t num_atoms_c = 0, axis_stride_c = 0; DevBuf<float> d_mass_c, d_init_c;
     uint32_t ingest_mode = 0, ingest_threads = 0; IngestPool* pool = nullptr;
     std::vector<uint32_t> conn_off; std::vector<int32_t> conn_idx;
     std::vector<Prop> props;
     std::vector<Slot> slots;
-    bool have_init = false; float* d_init = nullptr; mdgpu_unitcell_t init_cell{};
+    bool have_init = false; DevBuf<float> d_init; mdgpu_unitcell_t init_cell{};
     std::vector<uint64_t> frame_mask; std::mutex mask_mutex; std::mutex init_mutex;
     std::atomic<bool> interrupt{false};
     uint64_t next_slot = 0;
@@ -190,11 +261,11 @@ struct mdgpu_plan {
     // a caller thread owns a slot from acquire_slot to release_slot (staging buffers + stream); enqueue_batch runs under submit_mutex;
     // one fold at a time (sync_mutex).
     std::mutex slot_mutex; std::condition_variable slot_cv; std::mutex submit_mutex; std::mutex sync_mutex;
-    mdgpu_progress_fn progress_fn = nullptr; void* progress_user = nullptr; cudaStream_t pub_stream = nullptr;
+    mdgpu_progress_fn progress_fn = nullptr; void* progress_user = nullptr; Stream pub_stream;
     std::chrono::steady_clock::time_point last_pub{};
-    bool timing = false; std::vector<TimedLaunch> timed; double timed_ms[TIMED_KINDS] = {0, 0, 0, 0}; uint64_t timed_n[TIMED_KINDS] = {0, 0, 0, 0}; unsigned long long* d_counters = nullptr;
+    bool timing = false; std::vector<TimedLaunch> timed; double timed_ms[TIMED_KINDS] = {0, 0, 0, 0}; uint64_t timed_n[TIMED_KINDS] = {0, 0, 0, 0}; DevBuf<unsigned long long> d_counters;
     bool tri_seen = false, ortho_seen = false;
-    cudaEvent_t t_begin = nullptr; std::vector<cudaEvent_t> t_end;
+    Event t_begin; std::vector<Event> t_end;
     XtcStage xtc[XTC_STAGES]; uint64_t next_xtc = 0; std::mutex xtc_mutex;
     std::atomic<bool> dirty{true};   // device accumulators changed since the last fold into the host-visible property data
     std::atomic<uint64_t> frames_retired{0};   // frame evaluations of retired batches: the divisor of the running means
@@ -203,18 +274,6 @@ struct mdgpu_plan {
 
 // get_spatial_acc (md_script_functions.inl:734-760): the system-wide grid of within() has cells of ceil(radius / 6) * 6
 static double within_cell_ext(float radius) { return ceil((double)radius / 6.0) * 6.0; }
-
-static int alloc_cell_list(CellList& cl, uint32_t B, uint32_t max_points, uint32_t cap) {
-    cl.max_points = max_points; cl.cap = cap;
-    CUDA_TRY(dalloc(&cl.sorted, (size_t)B * max_points));
-    CUDA_TRY(dalloc(&cl.scratch, (size_t)B * max_points));
-    CUDA_TRY(dalloc(&cl.cell_of, (size_t)B * max_points));
-    CUDA_TRY(dalloc(&cl.rank, (size_t)B * max_points));
-    CUDA_TRY(dalloc(&cl.cell_cnt, (size_t)B * (cap + 1) + B));
-    cl.oob = cl.cell_cnt + (size_t)B * (cap + 1);
-    return 0;
-}
-static void free_cell_list(CellList& cl) { cudaFree(cl.sorted); cudaFree(cl.scratch); cudaFree(cl.cell_of); cudaFree(cl.rank); cudaFree(cl.cell_cnt); cl = CellList{}; }
 
 // BFS order in which md_util_unwrap_vec4(xyzw, NULL, count, bond, cell) visits atoms (md_util.c:8738-8819). NB the reference
 // walks the bonds of GLOBAL atoms 0..count-1 there (the local index is used as a global atom index); reproduced as is.
@@ -299,42 +358,43 @@ static inline void gather_axis(float* __restrict__ dst, const float* __restrict_
 static void destroy_multi(mdgpu_plan* p);
 static void destroy_plan(mdgpu_plan* p) {
     if (!p) return;
-    if (p->multi) destroy_multi(p);
-    cudaSetDevice(p->device);
+    if (p->multi) destroy_multi(p);   // the peers, each with its own device current
+    cudaSetDevice(p->device);         // the owners free this plan's buffers, streams and events on its device
     cudaDeviceSynchronize();
-    for (auto& s : p->slots) {
-        for (auto& ps : s.ps) {
-            cudaFree(ps.d_geom); cudaFree(ps.d_aabb); free_cell_list(ps.trg); free_cell_list(ps.ref);
-            cudaFree(ps.d_frame_bins); cudaFree(ps.d_frame_bins64); cudaFree(ps.d_sdf_xyzw); cudaFree(ps.d_sdf_ref0); cudaFree(ps.d_sdf_mats); cudaFree(ps.d_com); cudaFree(ps.d_argpos); cudaFree(ps.d_gpos[0]); cudaFree(ps.d_gpos[1]); for (auto* q : ps.d_parts) cudaFree(q); cudaFree(ps.d_flags); for (auto& w : ps.dynw) { cudaFree(w.d_geom); cudaFree(w.d_aabb); free_cell_list(w.trg); free_cell_list(w.ref); cudaFree(w.d_flags); cudaFree(w.d_idx); cudaFree(w.d_n); } cudaFree(ps.d_pair_list); cudaFree(ps.d_list_hdr); cudaFree(ps.d_list_cursor);
-            cudaFree(ps.d_poro_xyzr); cudaFree(ps.d_poro_hdr); cudaFree(ps.d_poro_grid); cudaFree(ps.d_poro_count);
-        }
-        cudaFree(s.d_frames); if (s.h_frames) cudaFreeHost(s.h_frames); cudaFree(s.d_xtc_frames);
-        cudaFree(s.d_cells); if (s.h_cells) cudaFreeHost(s.h_cells); cudaFree(s.d_err);
-        if (s.done) cudaEventDestroy(s.done);
-        if (s.copied) cudaEventDestroy(s.copied);
-        if (s.h_err) cudaFreeHost(s.h_err);
-        if (s.stream) cudaStreamDestroy(s.stream);
-    }
-    if (p->pub_stream) cudaStreamDestroy(p->pub_stream);
-    for (auto& st : p->xtc) {
-        cudaFree(st.d_blob); cudaFree(st.d_off); if (st.h_off) cudaFreeHost(st.h_off); cudaFree(st.d_info); cudaFree(st.d_rec); cudaFree(st.d_state);
-        if (st.ready) cudaEventDestroy(st.ready);
-        for (auto& e : st.consumed) if (e) cudaEventDestroy(e);
-        if (st.stream) cudaStreamDestroy(st.stream);
-    }
-    for (auto& pr : p->props) {
-        for (int k = 0; k < 4; ++k) { cudaFree(pr.d_idx[k]); cudaFree(pr.d_idx_c[k]); }
-        if (pr.values_registered) cudaHostUnregister(pr.values.data());
-        cudaFree(pr.d_vol_mean);
-        cudaFree(pr.d_acc); cudaFree(pr.d_vol); cudaFree(pr.d_frame_total); cudaFree(pr.d_frame_min); cudaFree(pr.d_frame_max);
-        cudaFree(pr.d_frame_min64); cudaFree(pr.d_frame_max64); cudaFree(pr.d_keep); cudaFree(pr.d_keep64); cudaFree(pr.d_temporal); cudaFree(pr.d_unwrap); cudaFree(pr.d_soff); cudaFree(pr.d_and_mask); cudaFree(pr.d_goff[0]); cudaFree(pr.d_goff[1]); for (auto* q : pr.d_aoff) cudaFree(q); cudaFree(pr.d_set_of); for (auto& dy : pr.dyn) cudaFree(dy.d_and_mask); cudaFree(pr.d_frame_n);
-    }
+    for (auto& pr : p->props) if (pr.values_registered) cudaHostUnregister(pr.values.data());
     for (auto& t : p->timed) { cudaEventDestroy(t.a); cudaEventDestroy(t.b); }
-    if (p->t_begin) cudaEventDestroy(p->t_begin);
-    for (auto e : p->t_end) cudaEventDestroy(e);
-    cudaFree(p->d_mass); cudaFree(p->d_radius); cudaFree(p->d_radius_c); cudaFree(p->d_init); cudaFree(p->d_mass_c); cudaFree(p->d_init_c); cudaFree(p->d_counters);
     delete p->pool;
     delete p;
+}
+
+// CSR offsets off[0..n] of groups in a list of `size` entries start at 0, end at the list's size and do not decrease: "" or the error message
+static std::string check_offsets(const uint32_t* off, size_t n, size_t size, const std::string& who, const char* noun, const char* list) {
+    if (!off || off[0] != 0u || off[n] != size) return who + ": " + noun + " do not cover " + list;
+    for (size_t g = 0; g < n; ++g) if (off[g] > off[g + 1]) return who + ": " + noun + " must be non-decreasing";
+    return std::string();
+}
+
+// the num_structures groups of idx[0]: structure_offsets, or runs of structure_size atoms -> pr.h_soff, checked; "" or the error message
+static std::string take_structures(Prop& pr, const mdgpu_property_desc_t& d, const std::string& who) {
+    if (d.structure_offsets) pr.h_soff.assign(d.structure_offsets, d.structure_offsets + pr.n_struct + 1);
+    else if (!pr.struct_size) return who + ": structure_size or structure_offsets required";
+    else { pr.h_soff.resize(pr.n_struct + 1); for (size_t k = 0; k <= pr.n_struct; ++k) pr.h_soff[k] = (uint32_t)(k * pr.struct_size); }
+    return check_offsets(pr.h_soff.data(), pr.n_struct, pr.h_idx[0].size(), who, "structure offsets", "idx[0]");
+}
+
+// a temporal of `len` values per frame: device rows, host values and, for len > 1, the per-frame aggregates (allocate_property_data :5618-5640)
+static cudaError_t set_temporal(Prop& pr, size_t num_frames, size_t len) {
+    pr.len = len;
+    pr.values.assign(num_frames * len, 0.0f);
+    if (len > 1) { pr.agg_mean.assign(num_frames, 0.0f); pr.agg_var.assign(num_frames, 0.0f); pr.agg_ext.assign(2 * num_frames, 0.0f); }
+    pr.data.dim[0] = (int32_t)num_frames; pr.data.dim[1] = (int32_t)len; pr.data.dim[2] = 0; pr.data.dim[3] = 0;
+    return pr.d_temporal.alloc(num_frames * len);
+}
+
+// a distribution (rdf, density): 1024 values followed by 1024 weights
+static void set_distribution(Prop& pr) {
+    pr.values.assign(2 * MDGPU_DIST_BINS, 0.0f);
+    pr.data.dim[0] = 1; pr.data.dim[1] = 2; pr.data.dim[2] = MDGPU_DIST_BINS; pr.data.dim[3] = 0;
 }
 
 extern "C" {
@@ -399,10 +459,9 @@ mdgpu_plan* mdgpu_plan_create(const mdgpu_system_desc_t* sys, const mdgpu_proper
             cnt[k] = pr.h_idx[k].size();
             if (!gn[k]) continue;
             if (pr.dyn[k].on) return "'" + pr.name + "': an array of selections cannot be a dynamic argument";
-            if (!goff[k] || goff[k][0] != 0 || goff[k][gn[k]] != pr.h_idx[k].size()) return "'" + pr.name + "': group offsets do not cover the index list";
-            for (size_t g = 0; g < gn[k]; ++g) if (goff[k][g] > goff[k][g + 1]) return "'" + pr.name + "': group offsets must be non-decreasing";
+            const std::string er = check_offsets(goff[k], gn[k], pr.h_idx[k].size(), "'" + pr.name + "'", "group offsets", "the index list"); if (!er.empty()) return er;
             pr.h_goff[k].assign(goff[k], goff[k] + gn[k] + 1); cnt[k] = gn[k];
-            if (upload(&pr.d_goff[k], pr.h_goff[k].data(), pr.h_goff[k].size()) != cudaSuccess) return "device allocation failed (group offsets)";
+            if (pr.d_goff[k].upload(pr.h_goff[k].data(), pr.h_goff[k].size()) != cudaSuccess) return "device allocation failed (group offsets)";
         }
         pr.n_struct = 0;   // num_structures described argument 0's groups here, not structures
         return std::string();
@@ -411,19 +470,18 @@ mdgpu_plan* mdgpu_plan_create(const mdgpu_system_desc_t* sys, const mdgpu_proper
     auto take_arg_parts = [&](Prop& pr, const mdgpu_property_desc_t& d, int k) -> std::string {
         const uint32_t n = d.arg_parts[k]; const uint32_t* off = d.arg_offsets[k];
         if (pr.dyn[k].on) return "'" + pr.name + "': an array of selections cannot be a dynamic argument";
-        if (!off || off[0] != 0u || off[n] != pr.h_idx[k].size()) return "'" + pr.name + "': argument offsets do not cover the index list";
-        for (uint32_t g = 0; g < n; ++g) if (off[g] > off[g + 1]) return "'" + pr.name + "': argument offsets must be non-decreasing";
+        const std::string er = check_offsets(off, n, pr.h_idx[k].size(), "'" + pr.name + "'", "argument offsets", "the index list"); if (!er.empty()) return er;
         pr.h_aoff[k].assign(off, off + n + 1);
-        if (upload(&pr.d_aoff[k], pr.h_aoff[k].data(), pr.h_aoff[k].size()) != cudaSuccess) return "device allocation failed (argument offsets)";
+        if (pr.d_aoff[k].upload(pr.h_aoff[k].data(), pr.h_aoff[k].size()) != cudaSuccess) return "device allocation failed (argument offsets)";
         pr.com_mask |= 1u << k;
         return std::string();
     };
-    if (upload(&p->d_mass, p->h_mass.data(), p->h_mass.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (masses)");
+    if (p->d_mass.upload(p->h_mass.data(), p->h_mass.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (masses)");
     for (size_t i = 0; i < num_props; ++i) if (props[i].op == MDGPU_OP_POROSITY) {   // porosity voxelises van der Waals spheres: the radii are required
         if (!sys->atom_radius) return bail(MDGPU_ERR_INVALID_ARG, "porosity: the system description has no atom radii (mdgpu_system_desc_t.atom_radius)");
         p->h_radius.assign(sys->atom_radius, sys->atom_radius + sys->num_atoms);
         for (size_t a = 0; a < sys->num_atoms; ++a) if (!(p->h_radius[a] >= 0.0f && p->h_radius[a] <= FLT_MAX)) return bail(MDGPU_ERR_INVALID_ARG, "porosity: atom radius " + std::to_string(a) + " is negative or not finite");
-        if (upload(&p->d_radius, p->h_radius.data(), p->h_radius.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (radii)");
+        if (p->d_radius.upload(p->h_radius.data(), p->h_radius.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (radii)");
         break;
     }
 
@@ -436,7 +494,7 @@ mdgpu_plan* mdgpu_plan_create(const mdgpu_system_desc_t* sys, const mdgpu_proper
             if (d.idx[k] && d.idx_count[k]) {
                 pr.h_idx[k].assign(d.idx[k], d.idx[k] + d.idx_count[k]);
                 for (int32_t a : pr.h_idx[k]) if ((a < 0 && !(pr.op == MDGPU_OP_BACKBONE_ANGLES && a == -1)) || (a >= 0 && (size_t)a >= sys->num_atoms)) return bail(MDGPU_ERR_INVALID_ARG, "property '" + pr.name + "': atom index out of range");
-                if (upload(&pr.d_idx[k], pr.h_idx[k].data(), pr.h_idx[k].size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (indices)");
+                if (pr.d_idx[k].upload(pr.h_idx[k].data(), pr.h_idx[k].size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (indices)");
             }
         }
         {   // dynamic arguments (dyn[k]); rdf's round-1 spelling ref_within_radius + com_args bit 0 + idx[2] becomes dyn[0]
@@ -455,13 +513,13 @@ mdgpu_plan* mdgpu_plan_create(const mdgpu_system_desc_t* sys, const mdgpu_proper
                 if (da[k].has_and) {
                     std::vector<uint8_t> m(sys->num_atoms, 0);
                     for (size_t j = 0; j < da[k].and_count; ++j) { const int32_t a = da[k].and_idx[j]; if (a < 0 || (size_t)a >= sys->num_atoms) return bail(MDGPU_ERR_INVALID_ARG, "property '" + pr.name + "': atom index out of range"); m[(size_t)a] = 1; }
-                    if (upload(&pr.dyn[k].d_and_mask, m.data(), m.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (selection mask)");
+                    if (pr.dyn[k].d_and_mask.upload(m.data(), m.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (selection mask)");
                 }
             }
         }
         if (pr.op == MDGPU_OP_WITHIN_COUNT && (d.com_args & 1u)) {   // idx[2] = static side of `sel and within(...)`
             std::vector<uint8_t> m(sys->num_atoms, 0); for (int32_t a : pr.h_idx[2]) m[(size_t)a] = 1;
-            if (upload(&pr.d_and_mask, m.data(), m.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (selection mask)");
+            if (pr.d_and_mask.upload(m.data(), m.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (selection mask)");
         }
         cudaError_t e = cudaSuccess;
         switch (pr.op) {
@@ -472,28 +530,22 @@ mdgpu_plan* mdgpu_plan_create(const mdgpu_system_desc_t* sys, const mdgpu_proper
             pr.ref_within = pr.dyn[0].on ? pr.dyn[0].rmax : 0.0f; pr.ref_within_min = pr.dyn[0].rmin;
             if (d.ref_within_radius < 0.0f || (pr.dyn[0].on && pr.n_struct) || d.ref_within_min < 0.0f) return bail(MDGPU_ERR_INVALID_ARG, "rdf '" + pr.name + "': invalid within() reference");
             if (pr.n_struct) {   // references = centres of mass of atom groups, a group's own atoms excluded (compute_rdf :5274-5275)
-                if (d.structure_offsets) pr.h_soff.assign(d.structure_offsets, d.structure_offsets + pr.n_struct + 1);
-                else { if (!pr.struct_size) return bail(MDGPU_ERR_INVALID_ARG, "rdf '" + pr.name + "': structure_size or structure_offsets required");
-                       pr.h_soff.resize(pr.n_struct + 1); for (size_t k = 0; k <= pr.n_struct; ++k) pr.h_soff[k] = (uint32_t)(k * pr.struct_size); }
-                if (pr.h_soff.front() != 0 || pr.h_soff.back() != pr.h_idx[0].size()) return bail(MDGPU_ERR_INVALID_ARG, "rdf '" + pr.name + "': structure offsets do not cover idx[0]");
-                for (size_t k = 0; k < pr.n_struct; ++k) if (pr.h_soff[k] > pr.h_soff[k + 1]) return bail(MDGPU_ERR_INVALID_ARG, "rdf '" + pr.name + "': structure offsets must be non-decreasing");
-                if (upload(&pr.d_soff, pr.h_soff.data(), pr.h_soff.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (structure offsets)");
+                const std::string er = take_structures(pr, d, "rdf '" + pr.name + "'"); if (!er.empty()) return bail(MDGPU_ERR_INVALID_ARG, er);
+                if (pr.d_soff.upload(pr.h_soff.data(), pr.h_soff.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (structure offsets)");
             }
             if (d.num_structures_b) {   // targets = centres of mass of atom groups (coordinate_extract :1503 -> extract_com :857 on an array of selections, compute_rdf :5293-5302)
                 const size_t n = d.num_structures_b; const uint32_t* off = d.structure_offsets_b;
                 if (pr.dyn[1].on) return bail(MDGPU_ERR_INVALID_ARG, "rdf '" + pr.name + "': an array of selections cannot be a dynamic target");
-                if (!off || off[0] != 0u || off[n] != pr.h_idx[1].size()) return bail(MDGPU_ERR_INVALID_ARG, "rdf '" + pr.name + "': target group offsets do not cover idx[1]");
-                for (size_t k = 0; k < n; ++k) if (off[k] > off[k + 1]) return bail(MDGPU_ERR_INVALID_ARG, "rdf '" + pr.name + "': target group offsets must be non-decreasing");
+                const std::string er = check_offsets(off, n, pr.h_idx[1].size(), "rdf '" + pr.name + "'", "target group offsets", "idx[1]"); if (!er.empty()) return bail(MDGPU_ERR_INVALID_ARG, er);
                 pr.h_goff[1].assign(off, off + n + 1); pr.trg_groups = n;
-                if (upload(&pr.d_goff[1], pr.h_goff[1].data(), pr.h_goff[1].size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (target group offsets)");
+                if (pr.d_goff[1].upload(pr.h_goff[1].data(), pr.h_goff[1].size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (target group offsets)");
             }
-            e = dalloc(&pr.d_acc, MDGPU_DIST_BINS);
-            if (e == cudaSuccess) e = dalloc(&pr.d_frame_total, num_frames);
-            if (e == cudaSuccess) e = dalloc(&pr.d_frame_min, num_frames);
-            if (e == cudaSuccess) e = dalloc(&pr.d_frame_max, num_frames);
-            if (e == cudaSuccess && p->keep) e = dalloc(&pr.d_keep, num_frames * MDGPU_DIST_BINS);
-            pr.values.assign(2 * MDGPU_DIST_BINS, 0.0f);
-            pr.data.dim[0] = 1; pr.data.dim[1] = 2; pr.data.dim[2] = MDGPU_DIST_BINS; pr.data.dim[3] = 0;
+            e = pr.d_acc.alloc(MDGPU_DIST_BINS);
+            if (e == cudaSuccess) e = pr.d_frame_total.alloc(num_frames);
+            if (e == cudaSuccess) e = pr.d_frame_min.alloc(num_frames);
+            if (e == cudaSuccess) e = pr.d_frame_max.alloc(num_frames);
+            if (e == cudaSuccess && p->keep) e = pr.d_keep.alloc(num_frames * MDGPU_DIST_BINS);
+            set_distribution(pr);
             break;
         case MDGPU_OP_SDF: {
             if (!pr.n_struct || !pr.struct_size || pr.h_idx[0].size() != pr.n_struct * pr.struct_size)
@@ -502,29 +554,26 @@ mdgpu_plan* mdgpu_plan_create(const mdgpu_system_desc_t* sys, const mdgpu_proper
             if (p->conn_off.empty()) return bail(MDGPU_ERR_INVALID_ARG, "sdf '" + pr.name + "': Missing bond connectivity");   // md_util.c:8746
             std::vector<int2> pairs; build_unwrap_pairs(pairs, pr.struct_size, p->conn_off, p->conn_idx);
             pr.n_unwrap = (uint32_t)pairs.size();
-            e = upload(&pr.d_unwrap, pairs.data(), pairs.size());
-            if (e == cudaSuccess) e = dalloc(&pr.d_vol, (size_t)MDGPU_VOL_DIM * MDGPU_VOL_DIM * MDGPU_VOL_DIM);
-            if (e == cudaSuccess) e = dalloc(&pr.d_vol_mean, (size_t)MDGPU_VOL_DIM * MDGPU_VOL_DIM * MDGPU_VOL_DIM);
-            if (e == cudaSuccess) e = dalloc(&pr.d_frame_total, num_frames);
+            e = pr.d_unwrap.upload(pairs.data(), pairs.size());
+            if (e == cudaSuccess) e = pr.d_vol.alloc((size_t)MDGPU_VOL_DIM * MDGPU_VOL_DIM * MDGPU_VOL_DIM);
+            if (e == cudaSuccess) e = pr.d_vol_mean.alloc((size_t)MDGPU_VOL_DIM * MDGPU_VOL_DIM * MDGPU_VOL_DIM);
+            if (e == cudaSuccess) e = pr.d_frame_total.alloc(num_frames);
             pr.values.assign((size_t)MDGPU_VOL_DIM * MDGPU_VOL_DIM * MDGPU_VOL_DIM, 0.0f);
             if (cudaHostRegister(pr.values.data(), pr.values.size() * sizeof(float), cudaHostRegisterDefault) == cudaSuccess) pr.values_registered = true; else cudaGetLastError();
             pr.data.dim[0] = 1; pr.data.dim[1] = MDGPU_VOL_DIM; pr.data.dim[2] = MDGPU_VOL_DIM; pr.data.dim[3] = MDGPU_VOL_DIM;
             break; }
         case MDGPU_OP_DENSITY_X: case MDGPU_OP_DENSITY_Y: case MDGPU_OP_DENSITY_Z:
             if (pr.h_idx[0].empty() && !pr.dyn[0].on) return bail(MDGPU_ERR_INVALID_ARG, "density '" + pr.name + "': empty selection");
-            e = dalloc(&pr.d_acc, MDGPU_DIST_BINS);
-            if (e == cudaSuccess) e = dalloc(&pr.d_frame_min64, num_frames);
-            if (e == cudaSuccess) e = dalloc(&pr.d_frame_max64, num_frames);
-            if (e == cudaSuccess && p->keep) e = dalloc(&pr.d_keep64, num_frames * MDGPU_DIST_BINS);
-            pr.values.assign(2 * MDGPU_DIST_BINS, 0.0f);
-            pr.data.dim[0] = 1; pr.data.dim[1] = 2; pr.data.dim[2] = MDGPU_DIST_BINS; pr.data.dim[3] = 0;
+            e = pr.d_acc.alloc(MDGPU_DIST_BINS);
+            if (e == cudaSuccess) e = pr.d_frame_min64.alloc(num_frames);
+            if (e == cudaSuccess) e = pr.d_frame_max64.alloc(num_frames);
+            if (e == cudaSuccess && p->keep) e = pr.d_keep64.alloc(num_frames * MDGPU_DIST_BINS);
+            set_distribution(pr);
             break;
         case MDGPU_OP_DISTANCE_MIN: case MDGPU_OP_DISTANCE_MAX:
             if ((pr.h_idx[0].empty() && !pr.dyn[0].on) || (pr.h_idx[1].empty() && !pr.dyn[1].on)) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': empty argument");
             { size_t cnt[2]; const std::string er = take_groups(pr, d, cnt); if (!er.empty()) return bail(MDGPU_ERR_INVALID_ARG, er); }   // arrays of selections: one centre of mass per selection
-            e = dalloc(&pr.d_temporal, num_frames);
-            pr.values.assign(num_frames, 0.0f);
-            pr.data.dim[0] = (int32_t)num_frames; pr.data.dim[1] = 1; pr.data.dim[2] = 0; pr.data.dim[3] = 0;
+            e = set_temporal(pr, num_frames, 1);
             break;
         case MDGPU_OP_DISTANCE: case MDGPU_OP_ANGLE: case MDGPU_OP_DIHEDRAL: {
             const int need = pr.op == MDGPU_OP_DISTANCE ? 2 : (pr.op == MDGPU_OP_ANGLE ? 3 : 4);
@@ -538,11 +587,7 @@ mdgpu_plan* mdgpu_plan_create(const mdgpu_system_desc_t* sys, const mdgpu_proper
                         const std::string er = take_arg_parts(pr, d, k); if (!er.empty()) return bail(MDGPU_ERR_INVALID_ARG, er);
                     } else if (pr.h_idx[k].size() != pr.n_struct) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': one atom per context and argument expected");
                 }
-                pr.len = pr.n_struct;
-                e = dalloc(&pr.d_temporal, num_frames * pr.len);
-                pr.values.assign(num_frames * pr.len, 0.0f);
-                if (pr.len > 1) { pr.agg_mean.assign(num_frames, 0.0f); pr.agg_var.assign(num_frames, 0.0f); pr.agg_ext.assign(2 * num_frames, 0.0f); }
-                pr.data.dim[0] = (int32_t)num_frames; pr.data.dim[1] = (int32_t)pr.len; pr.data.dim[2] = 0; pr.data.dim[3] = 0;
+                e = set_temporal(pr, num_frames, pr.n_struct);
                 break;
             }
             pr.com_mask = d.com_args & ((1u << need) - 1u);
@@ -552,62 +597,39 @@ mdgpu_plan* mdgpu_plan_create(const mdgpu_system_desc_t* sys, const mdgpu_proper
                 if (pr.h_idx[k].empty()) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': empty argument");
                 if (pr.h_idx[k].size() != 1) pr.com_mask |= 1u << k;   // several indices: centre of mass (coordinate_extract_com :1759)
             }
-            e = dalloc(&pr.d_temporal, num_frames);
-            pr.values.assign(num_frames, 0.0f);
-            pr.data.dim[0] = (int32_t)num_frames; pr.data.dim[1] = 1; pr.data.dim[2] = 0; pr.data.dim[3] = 0;
+            e = set_temporal(pr, num_frames, 1);
             break; }
         case MDGPU_OP_DISTANCE_PAIR: {
             if (pr.h_idx[0].empty() || pr.h_idx[1].empty()) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': empty argument");
             // an argument that was an ARRAY of selections contributes one position per selection: extract_com (:857, no periodic treatment; coordinate_extract :1503)
             size_t cnt[2];
             { const std::string er = take_groups(pr, d, cnt); if (!er.empty()) return bail(MDGPU_ERR_INVALID_ARG, er); }
-            pr.len = cnt[0] * cnt[1];
-            if (pr.len > 1000000) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': The size produced by the operation is " + std::to_string(pr.len) + ", which exceeds the upper limit of 1'000'000");   // :4056
-            e = dalloc(&pr.d_temporal, num_frames * pr.len);
-            pr.values.assign(num_frames * pr.len, 0.0f);
-            if (pr.len > 1) { pr.agg_mean.assign(num_frames, 0.0f); pr.agg_var.assign(num_frames, 0.0f); pr.agg_ext.assign(2 * num_frames, 0.0f); }   // allocate_property_data :5618-5640
-            pr.data.dim[0] = (int32_t)num_frames; pr.data.dim[1] = (int32_t)pr.len; pr.data.dim[2] = 0; pr.data.dim[3] = 0;
+            const size_t len = cnt[0] * cnt[1];
+            if (len > 1000000) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': The size produced by the operation is " + std::to_string(len) + ", which exceeds the upper limit of 1'000'000");   // :4056
+            e = set_temporal(pr, num_frames, len);
             break; }
         case MDGPU_OP_WITHIN_COUNT:   // count(within(radius, selection)); an empty selection is valid (nothing is within reach of nothing)
             if (!(pr.cutoff_max > 0.0f)) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': The supplied radius is negative or zero, please supply a positive value");   // :2528
             if (pr.cutoff_min < 0.0f || pr.cutoff_max < pr.cutoff_min) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': The supplied radius range is invalid");          // :2654
-            e = dalloc(&pr.d_temporal, num_frames);
-            pr.values.assign(num_frames, 0.0f);
-            pr.data.dim[0] = (int32_t)num_frames; pr.data.dim[1] = 1; pr.data.dim[2] = 0; pr.data.dim[3] = 0;
+            e = set_temporal(pr, num_frames, 1);
             break;
         case MDGPU_OP_SHAPE_WEIGHTS: {   // shape weights of n structures: [F, n*3]; groups as for rdf's centre-of-mass references
             if (!pr.n_struct || pr.h_idx[0].empty()) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': No structures present");   // shapespace.cpp:371
-            if (d.structure_offsets) pr.h_soff.assign(d.structure_offsets, d.structure_offsets + pr.n_struct + 1);
-            else { if (!pr.struct_size) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': structure_size or structure_offsets required");
-                   pr.h_soff.resize(pr.n_struct + 1); for (size_t k = 0; k <= pr.n_struct; ++k) pr.h_soff[k] = (uint32_t)(k * pr.struct_size); }
-            if (pr.h_soff.front() != 0 || pr.h_soff.back() != pr.h_idx[0].size()) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': structure offsets do not cover idx[0]");
-            for (size_t k = 0; k < pr.n_struct; ++k) if (pr.h_soff[k] > pr.h_soff[k + 1]) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': structure offsets must be non-decreasing");
-            if (upload(&pr.d_soff, pr.h_soff.data(), pr.h_soff.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (structure offsets)");
+            { const std::string er = take_structures(pr, d, "'" + pr.name + "'"); if (!er.empty()) return bail(MDGPU_ERR_INVALID_ARG, er); }
+            if (pr.d_soff.upload(pr.h_soff.data(), pr.h_soff.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (structure offsets)");
             pr.com_mask = d.com_args & 1u;   // bit 0: weights are the atom masses (else 1)
-            pr.len = 3 * pr.n_struct;
-            e = dalloc(&pr.d_temporal, num_frames * pr.len);
-            pr.values.assign(num_frames * pr.len, 0.0f);
-            pr.agg_mean.assign(num_frames, 0.0f); pr.agg_var.assign(num_frames, 0.0f); pr.agg_ext.assign(2 * num_frames, 0.0f);
-            pr.data.dim[0] = (int32_t)num_frames; pr.data.dim[1] = (int32_t)pr.len; pr.data.dim[2] = 0; pr.data.dim[3] = 0;
+            e = set_temporal(pr, num_frames, 3 * pr.n_struct);
             break; }
         case MDGPU_OP_COORD_X: case MDGPU_OP_COORD_Y: case MDGPU_OP_COORD_Z:   // coord_x/_y/_z(selection): [F, n]
             if (pr.h_idx[0].empty()) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': empty argument");
             { size_t cnt[2]; const std::string er = take_groups(pr, d, cnt); if (!er.empty()) return bail(MDGPU_ERR_INVALID_ARG, er);   // an array of selections: one value per selection
-              pr.len = cnt[0]; }
-            e = dalloc(&pr.d_temporal, num_frames * pr.len);
-            pr.values.assign(num_frames * pr.len, 0.0f);
-            if (pr.len > 1) { pr.agg_mean.assign(num_frames, 0.0f); pr.agg_var.assign(num_frames, 0.0f); pr.agg_ext.assign(2 * num_frames, 0.0f); }
-            pr.data.dim[0] = (int32_t)num_frames; pr.data.dim[1] = (int32_t)pr.len; pr.data.dim[2] = 0; pr.data.dim[3] = 0;
+              e = set_temporal(pr, num_frames, cnt[0]); }
             break;
         case MDGPU_OP_COM: {   // com(x): a [F, 3] temporal (TI_FLOAT3)
             if (pr.h_idx[0].empty() && !pr.dyn[0].on) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': empty argument");
             pr.com_mask = (d.com_args & 1u) | (pr.h_idx[0].size() != 1 ? 1u : 0u) | (pr.dyn[0].on ? 1u : 0u);
             if (d.arg_parts[0] > 1u) { const std::string er = take_arg_parts(pr, d, 0); if (!er.empty()) return bail(MDGPU_ERR_INVALID_ARG, er); }
-            pr.len = 3;
-            e = dalloc(&pr.d_temporal, num_frames * pr.len);
-            pr.values.assign(num_frames * pr.len, 0.0f);
-            pr.agg_mean.assign(num_frames, 0.0f); pr.agg_var.assign(num_frames, 0.0f); pr.agg_ext.assign(2 * num_frames, 0.0f);
-            pr.data.dim[0] = (int32_t)num_frames; pr.data.dim[1] = 3; pr.data.dim[2] = 0; pr.data.dim[3] = 0;
+            e = set_temporal(pr, num_frames, 3);
             break; }
         case MDGPU_OP_PLANE: {   // plane(selection): a [F, 4] temporal (TI_FLOAT4)
             size_t cnt[2];   // an array of selections: its positions are the selections' centres of mass (coordinate_extract :1503)
@@ -616,36 +638,25 @@ mdgpu_plan* mdgpu_plan_create(const mdgpu_system_desc_t* sys, const mdgpu_proper
             // md_util_unwrap_vec4 is called without indices (:4771): position i is unwrapped along the bonds of ATOM i, whatever was selected — as written
             std::vector<int2> pairs; build_unwrap_pairs(pairs, cnt[0], p->conn_off, p->conn_idx);
             pr.n_unwrap = (uint32_t)pairs.size();
-            e = upload(&pr.d_unwrap, pairs.data(), pairs.size());
-            pr.len = 4;
-            if (e == cudaSuccess) e = dalloc(&pr.d_temporal, num_frames * pr.len);
-            pr.values.assign(num_frames * pr.len, 0.0f);
-            pr.agg_mean.assign(num_frames, 0.0f); pr.agg_var.assign(num_frames, 0.0f); pr.agg_ext.assign(2 * num_frames, 0.0f);
-            pr.data.dim[0] = (int32_t)num_frames; pr.data.dim[1] = 4; pr.data.dim[2] = 0; pr.data.dim[3] = 0;
+            e = pr.d_unwrap.upload(pairs.data(), pairs.size());
+            if (e == cudaSuccess) e = set_temporal(pr, num_frames, 4);
             break; }
         case MDGPU_OP_CONTACT_COUNT: {   // contact_count(A[], B, cutoff): per set the pairs (a in A_i, b in B) within the cutoff, b outside the set's exclusion list
             if (!pr.n_struct || pr.h_idx[0].empty()) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': no sets");
             if (pr.n_struct > MDGPU_DIST_BINS) return bail(MDGPU_ERR_UNSUPPORTED, "'" + pr.name + "': more than 1024 sets");
             if (!(pr.cutoff_max > 0.0f)) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': The cutoff distance must be positive.");   // :2862
             if (pr.h_idx[1].empty()) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': empty second set");
-            if (d.structure_offsets) pr.h_soff.assign(d.structure_offsets, d.structure_offsets + pr.n_struct + 1);
-            else { if (!pr.struct_size) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': structure_size or structure_offsets required");
-                   pr.h_soff.resize(pr.n_struct + 1); for (size_t k = 0; k <= pr.n_struct; ++k) pr.h_soff[k] = (uint32_t)(k * pr.struct_size); }
-            if (pr.h_soff.front() != 0 || pr.h_soff.back() != pr.h_idx[0].size()) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': structure offsets do not cover idx[0]");
+            { const std::string er = take_structures(pr, d, "'" + pr.name + "'"); if (!er.empty()) return bail(MDGPU_ERR_INVALID_ARG, er); }
             std::vector<uint32_t> set_of(pr.h_idx[0].size());
-            for (size_t k = 0; k < pr.n_struct; ++k) { if (pr.h_soff[k] > pr.h_soff[k + 1]) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': structure offsets must be non-decreasing"); for (uint32_t j = pr.h_soff[k]; j < pr.h_soff[k + 1]; ++j) set_of[j] = (uint32_t)k; }
+            for (size_t k = 0; k < pr.n_struct; ++k) for (uint32_t j = pr.h_soff[k]; j < pr.h_soff[k + 1]; ++j) set_of[j] = (uint32_t)k;
             // exclusion lists (A_i & B grown along the bonds, md_util_mask_grow_by_bonds): CSR in idx[2] / structure_offsets_b, empty when absent
             pr.h_goff[1].assign(pr.n_struct + 1, 0u);
             if (d.structure_offsets_b) { if (d.num_structures_b != pr.n_struct || d.structure_offsets_b[0] != 0 || d.structure_offsets_b[pr.n_struct] != pr.h_idx[2].size()) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': exclusion offsets do not cover idx[2]");
                                          pr.h_goff[1].assign(d.structure_offsets_b, d.structure_offsets_b + pr.n_struct + 1); }
             else if (!pr.h_idx[2].empty()) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': exclusion atoms without offsets");
-            e = upload(&pr.d_set_of, set_of.data(), set_of.size());
-            if (e == cudaSuccess) e = upload(&pr.d_goff[1], pr.h_goff[1].data(), pr.h_goff[1].size());
-            pr.len = pr.n_struct;
-            if (e == cudaSuccess) e = dalloc(&pr.d_temporal, num_frames * pr.len);
-            pr.values.assign(num_frames * pr.len, 0.0f);
-            if (pr.len > 1) { pr.agg_mean.assign(num_frames, 0.0f); pr.agg_var.assign(num_frames, 0.0f); pr.agg_ext.assign(2 * num_frames, 0.0f); }
-            pr.data.dim[0] = (int32_t)num_frames; pr.data.dim[1] = (int32_t)pr.len; pr.data.dim[2] = 0; pr.data.dim[3] = 0;
+            e = pr.d_set_of.upload(set_of.data(), set_of.size());
+            if (e == cudaSuccess) e = pr.d_goff[1].upload(pr.h_goff[1].data(), pr.h_goff[1].size());
+            if (e == cudaSuccess) e = set_temporal(pr, num_frames, pr.n_struct);
             break; }
         case MDGPU_OP_BACKBONE_ANGLES: {   // two `dihedral in context` values per segment: phi = (C', N, CA, C), psi = (N, CA, C, N')
             const size_t ns = pr.n_struct;
@@ -659,30 +670,23 @@ mdgpu_plan* mdgpu_plan_create(const mdgpu_system_desc_t* sys, const mdgpu_proper
                 for (int k = 0; k < 4; ++k) { ctx[k][2 * i] = ok ? q[k] : -1; ctx[k][2 * i + 1] = ok ? q[k + 1] : -1; }
             }
             for (int k = 0; k < 4; ++k) {
-                cudaFree(pr.d_idx[k]); pr.d_idx[k] = nullptr; pr.h_idx[k] = ctx[k];
-                if (upload(&pr.d_idx[k], pr.h_idx[k].data(), pr.h_idx[k].size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (indices)");
+                pr.d_idx[k].reset(); pr.h_idx[k] = ctx[k];
+                if (pr.d_idx[k].upload(pr.h_idx[k].data(), pr.h_idx[k].size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (indices)");
             }
-            pr.op = MDGPU_OP_DIHEDRAL; pr.n_struct = 2 * ns; pr.len = 2 * ns; pr.backbone_segments = ns;
-            e = dalloc(&pr.d_temporal, num_frames * pr.len);
-            pr.values.assign(num_frames * pr.len, 0.0f);
-            pr.agg_mean.assign(num_frames, 0.0f); pr.agg_var.assign(num_frames, 0.0f); pr.agg_ext.assign(2 * num_frames, 0.0f);
-            pr.data.dim[0] = (int32_t)num_frames; pr.data.dim[1] = (int32_t)pr.len; pr.data.dim[2] = 0; pr.data.dim[3] = 0;
+            pr.op = MDGPU_OP_DIHEDRAL; pr.n_struct = 2 * ns; pr.backbone_segments = ns;
+            e = set_temporal(pr, num_frames, 2 * ns);
             break; }
         case MDGPU_OP_POROSITY:   // porosity(selection): [F, 1]; an empty selection is valid and evaluates to 0 (:5896-5899)
-            e = dalloc(&pr.d_temporal, num_frames);
-            if (e == cudaSuccess) e = dalloc(&pr.d_frame_total, num_frames);
-            if (e == cudaSuccess) e = dalloc(&pr.d_frame_n, num_frames);
-            pr.values.assign(num_frames, 0.0f);
-            pr.data.dim[0] = (int32_t)num_frames; pr.data.dim[1] = 1; pr.data.dim[2] = 0; pr.data.dim[3] = 0;
+            e = set_temporal(pr, num_frames, 1);
+            if (e == cudaSuccess) e = pr.d_frame_total.alloc(num_frames);
+            if (e == cudaSuccess) e = pr.d_frame_n.alloc(num_frames);
             break;
         case MDGPU_OP_RMSD: {   // an empty selection is valid and evaluates to 0 (_rmsd :4311, :4336-4338)
             std::vector<int2> pairs;   // without bonds md_util_unwrap_vec4 fails and its result is ignored (:4327): nothing is unwrapped
             build_unwrap_pairs(pairs, pr.h_idx[0].size(), p->conn_off, p->conn_idx);
             pr.n_unwrap = (uint32_t)pairs.size();
-            e = upload(&pr.d_unwrap, pairs.data(), pairs.size());
-            if (e == cudaSuccess) e = dalloc(&pr.d_temporal, num_frames);
-            pr.values.assign(num_frames, 0.0f);
-            pr.data.dim[0] = (int32_t)num_frames; pr.data.dim[1] = 1; pr.data.dim[2] = 0; pr.data.dim[3] = 0;
+            e = pr.d_unwrap.upload(pairs.data(), pairs.size());
+            if (e == cudaSuccess) e = set_temporal(pr, num_frames, 1);
             break; }
         default:
             return bail(MDGPU_ERR_UNSUPPORTED, "property '" + pr.name + "': unsupported operation " + std::to_string(pr.op));
@@ -711,46 +715,48 @@ mdgpu_plan* mdgpu_plan_create(const mdgpu_system_desc_t* sys, const mdgpu_proper
             std::vector<int32_t> map(N, -1); for (size_t j = 0; j < p->needed.size(); ++j) map[(size_t)p->needed[j]] = (int32_t)j;
             p->num_atoms_c = p->needed.size(); p->axis_stride_c = (p->num_atoms_c + 3) & ~(size_t)3;
             std::vector<float> mc(p->num_atoms_c); for (size_t j = 0; j < mc.size(); ++j) mc[j] = p->h_mass[(size_t)p->needed[j]];
-            if (upload(&p->d_mass_c, mc.data(), mc.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (masses)");
+            if (p->d_mass_c.upload(mc.data(), mc.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (masses)");
             if (!p->h_radius.empty()) {
                 std::vector<float> rc(p->num_atoms_c); for (size_t j = 0; j < rc.size(); ++j) rc[j] = p->h_radius[(size_t)p->needed[j]];
-                if (upload(&p->d_radius_c, rc.data(), rc.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (radii)");
+                if (p->d_radius_c.upload(rc.data(), rc.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (radii)");
             }
             for (auto& pr : p->props) for (int k = 0; k < 4; ++k) if (!pr.h_idx[k].empty()) {
                 std::vector<int32_t> ci(pr.h_idx[k].size()); for (size_t j = 0; j < ci.size(); ++j) ci[j] = pr.h_idx[k][j] < 0 ? -1 : map[(size_t)pr.h_idx[k][j]];
                 pr.first_c[k] = ci[0];
-                if (upload(&pr.d_idx_c[k], ci.data(), ci.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (indices)");
+                if (pr.d_idx_c[k].upload(ci.data(), ci.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (indices)");
             }
-            if (cudaMalloc((void**)&p->d_init_c, sizeof(float) * 3 * p->axis_stride_c) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (initial frame)");
+            if (p->d_init_c.alloc(3 * p->axis_stride_c) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (initial frame)");
         }
     }
     p->frame_mask.assign((num_frames + 63) / 64, 0);
-    if (cudaMalloc((void**)&p->d_init, sizeof(float) * 3 * p->axis_stride) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (initial frame)");
+    if (p->d_init.alloc(3 * p->axis_stride) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (initial frame)");
     if (mdgpu_plan_clear(p) != 0) { destroy_plan(p); return nullptr; }
     return p;
 }
 
 void mdgpu_plan_destroy(mdgpu_plan* plan) { destroy_plan(plan); }
 
+}  // extern "C"
+
+static int zero_accumulators(Prop& pr) {
+    return Prop::for_each_accumulator([&](auto member) -> int {
+        auto& b = pr.*member;
+        if (b.get()) CUDA_TRY(cudaMemset(b.get(), 0, b.bytes()));
+        return 0;
+    });
+}
+
+extern "C" {
+
 int mdgpu_plan_clear(mdgpu_plan* p) {
     if (!p) return fail(MDGPU_ERR_INVALID_ARG, "null plan");
     if (p->multi) for (auto* q : p->multi->peers) { int rc = mdgpu_plan_clear(q); if (rc) return rc; }
     CUDA_TRY(cudaSetDevice(p->device));
     CUDA_TRY(cudaDeviceSynchronize());
-    for (auto& s : p->slots) { s.busy = false; if (s.h_err) *s.h_err = 0; if (s.d_err) CUDA_TRY(cudaMemset(s.d_err, 0, sizeof(int))); }
+    for (auto& s : p->slots) { s.busy = false; s.h_err[0] = 0; CUDA_TRY(cudaMemset(s.d_err.get(), 0, sizeof(int))); }
     for (auto& pr : p->props) {
-        if (pr.d_acc) CUDA_TRY(cudaMemset(pr.d_acc, 0, sizeof(unsigned long long) * MDGPU_DIST_BINS));
-        if (pr.d_vol) CUDA_TRY(cudaMemset(pr.d_vol, 0, sizeof(uint32_t) * MDGPU_VOL_DIM * MDGPU_VOL_DIM * MDGPU_VOL_DIM));
-        if (pr.d_frame_total) CUDA_TRY(cudaMemset(pr.d_frame_total, 0, sizeof(unsigned long long) * p->num_frames));
-        if (pr.d_frame_n) CUDA_TRY(cudaMemset(pr.d_frame_n, 0, sizeof(unsigned long long) * p->num_frames));
-        if (pr.d_frame_min) CUDA_TRY(cudaMemset(pr.d_frame_min, 0, sizeof(uint32_t) * p->num_frames));
-        if (pr.d_frame_max) CUDA_TRY(cudaMemset(pr.d_frame_max, 0, sizeof(uint32_t) * p->num_frames));
-        if (pr.d_frame_min64) CUDA_TRY(cudaMemset(pr.d_frame_min64, 0, sizeof(unsigned long long) * p->num_frames));
-        if (pr.d_frame_max64) CUDA_TRY(cudaMemset(pr.d_frame_max64, 0, sizeof(unsigned long long) * p->num_frames));
-        if (pr.d_temporal) CUDA_TRY(cudaMemset(pr.d_temporal, 0, sizeof(float) * p->num_frames * pr.len));
+        { const int rc = zero_accumulators(pr); if (rc) return rc; }
         if (!pr.agg_mean.empty()) { std::fill(pr.amean, pr.amean + p->num_frames, 0.0f); std::fill(pr.avar, pr.avar + p->num_frames, 0.0f); std::fill(pr.aext, pr.aext + 2 * p->num_frames, 0.0f); }
-        if (pr.d_keep) CUDA_TRY(cudaMemset(pr.d_keep, 0, sizeof(uint32_t) * p->num_frames * MDGPU_DIST_BINS));
-        if (pr.d_keep64) CUDA_TRY(cudaMemset(pr.d_keep64, 0, sizeof(unsigned long long) * p->num_frames * MDGPU_DIST_BINS));
         std::fill(pr.vptr, pr.vptr + pr.values.size(), 0.0f);
         if (pr.is_dist()) std::fill(pr.vptr + MDGPU_DIST_BINS, pr.vptr + pr.values.size(), 1.0f);   // allocate_property_data :5613-5618
         pr.data.min_value = +FLT_MAX; pr.data.max_value = -FLT_MAX;                                 // clear_property_data :5726-5727
@@ -760,7 +766,7 @@ int mdgpu_plan_clear(mdgpu_plan* p) {
     { std::lock_guard<std::mutex> lk(p->mask_mutex); std::fill(p->frame_mask.begin(), p->frame_mask.end(), 0ull); }
     p->interrupt = false; p->frames_retired = 0;
     for (int k = 0; k < TIMED_KINDS; ++k) { p->timed_ms[k] = 0; p->timed_n[k] = 0; }
-    if (p->d_counters) CUDA_TRY(cudaMemset(p->d_counters, 0, sizeof(unsigned long long) * 8));
+    if (p->d_counters.get()) CUDA_TRY(cudaMemset(p->d_counters.get(), 0, p->d_counters.bytes()));
     p->dirty = true;
     return 0;
 }
@@ -769,13 +775,13 @@ int mdgpu_plan_set_initial_frame(mdgpu_plan* p, const float* x, const float* y, 
     if (!p || !x || !y || !z || !cell) return fail(MDGPU_ERR_INVALID_ARG, "mdgpu_plan_set_initial_frame: null argument");
     if (p->multi) for (auto* q : p->multi->peers) { int rc = mdgpu_plan_set_initial_frame(q, x, y, z, cell); if (rc) return rc; }
     CUDA_TRY(cudaSetDevice(p->device));
-    CUDA_TRY(cudaMemcpy(p->d_init, x, sizeof(float) * p->num_atoms, cudaMemcpyHostToDevice));
-    CUDA_TRY(cudaMemcpy(p->d_init + p->axis_stride, y, sizeof(float) * p->num_atoms, cudaMemcpyHostToDevice));
-    CUDA_TRY(cudaMemcpy(p->d_init + 2 * p->axis_stride, z, sizeof(float) * p->num_atoms, cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemcpy(p->d_init.get(), x, sizeof(float) * p->num_atoms, cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemcpy(p->d_init.get() + p->axis_stride, y, sizeof(float) * p->num_atoms, cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemcpy(p->d_init.get() + 2 * p->axis_stride, z, sizeof(float) * p->num_atoms, cudaMemcpyHostToDevice));
     if (p->compact) {
         std::vector<float> c(3 * p->axis_stride_c, 0.0f); const float* src[3] = { x, y, z };
         for (int ax = 0; ax < 3; ++ax) gather_axis(c.data() + (size_t)ax * p->axis_stride_c, src[ax], p->needed.data(), p->num_atoms_c);
-        CUDA_TRY(cudaMemcpy(p->d_init_c, c.data(), sizeof(float) * c.size(), cudaMemcpyHostToDevice));
+        CUDA_TRY(cudaMemcpy(p->d_init_c.get(), c.data(), sizeof(float) * c.size(), cudaMemcpyHostToDevice));
     }
     p->init_cell = *cell; p->have_init = true;
     for (auto& pr : p->props) {
@@ -799,8 +805,90 @@ int mdgpu_plan_set_initial_frame(mdgpu_plan* p, const float* x, const float* y, 
 }  // extern "C"
 
 // ---------------------------------------------------------------------------------------------------------------
-// slot set-up (lazy: needs the initial frame for the default cell capacity)
+// slot set-up
 // ---------------------------------------------------------------------------------------------------------------
+// rdf candidate lists of the packed pair kernel, entries per frame for frames of `cell`: every target appears in at most (2n+1)^3 home cells'
+// lists, n the neighbour reach of the cell (an NPT or sheared cell can cross from 27 to 125 offsets); a grid fitted to the data (AABB) gets
+// the widest reach the reference allows. A dynamic target set is sized for a quarter of the system; frames that select more are finished by
+// the overflow pass.
+static size_t rdf_list_stride(const mdgpu_plan* p, const Prop& pr, const mdgpu_unitcell_t* cell) {
+    FrameGeom g; host_frame_geom(&g, cell, pr.cutoff_max, pr.cutoff_max, nullptr, 0xffffffffu);
+    size_t nn = (size_t)(2 * std::max(g.ncell[0], 1) + 1) * (2 * std::max(g.ncell[1], 1) + 1) * (2 * std::max(g.ncell[2], 1) + 1);
+    if (g.valid <= 0 || (cell->flags & MDGPU_CELL_PBC_ALL) != MDGPU_CELL_PBC_ALL) nn = 125;
+    return std::min<size_t>(nn, 125) * (pr.dyn[1].on ? std::max<size_t>(p->num_atoms / 4, 1024) : pr.h_idx[1].size()) + 1024;
+}
+
+// One stream slot with the scratch of every property, for cell capacity `cap`.
+static int build_slot(mdgpu_plan* p, Slot& s, const mdgpu_unitcell_t* first_cell, uint32_t cap) {
+    CUDA_TRY(cudaStreamCreateWithFlags(s.stream.out(), cudaStreamNonBlocking));
+    CUDA_TRY(cudaEventCreateWithFlags(s.done.out(), cudaEventDisableTiming));
+    CUDA_TRY(cudaEventCreateWithFlags(s.copied.out(), cudaEventDisableTiming));
+    CUDA_TRY(s.h_err.alloc(1)); s.h_err[0] = 0;
+    CUDA_TRY(s.d_cells.alloc(p->B));
+    CUDA_TRY(s.h_cells.alloc(p->B));
+    CUDA_TRY(s.d_err.alloc(1)); CUDA_TRY(cudaMemset(s.d_err.get(), 0, sizeof(int)));
+    s.ps.resize(p->props.size());
+    for (size_t i = 0; i < p->props.size(); ++i) {
+        Prop& pr = p->props[i]; PropScratch& ps = s.ps[i];
+        for (int k = 0; k < 4; ++k) if (pr.dyn[k].on) {   // the within() query of a dynamic argument: system-wide lists + marks + per-frame index list
+            auto& w = ps.dynw[k];
+            CUDA_TRY(w.d_geom.alloc(p->B)); CUDA_TRY(w.d_aabb.alloc((size_t)6 * p->B));
+            CUDA_TRY(w.trg.alloc(p->B, (uint32_t)p->num_atoms, cap));
+            CUDA_TRY(w.ref.alloc(p->B, (uint32_t)std::max<size_t>(pr.h_idx[k].size(), 1), cap));
+            CUDA_TRY(w.d_flags.alloc((size_t)p->B * p->num_atoms));
+            CUDA_TRY(w.d_idx.alloc((size_t)p->B * p->num_atoms)); CUDA_TRY(w.d_n.alloc(p->B));
+        }
+        if (pr.needs_cells() && pr.share_trg < 0) {
+            CUDA_TRY(ps.d_geom.alloc(p->B)); CUDA_TRY(ps.d_aabb.alloc((size_t)6 * p->B));
+            CUDA_TRY(ps.trg.alloc(p->B, (uint32_t)(pr.dyn[1].on ? p->num_atoms : (pr.trg_groups ? pr.trg_groups : pr.h_idx[1].size())), cap));
+            if (pr.trg_groups) CUDA_TRY(ps.d_gpos[1].alloc((size_t)p->B * pr.trg_groups * 3));
+        }
+        if (pr.op == MDGPU_OP_RDF) {
+            CUDA_TRY(ps.ref.alloc(p->B, (uint32_t)(pr.dyn[0].on ? p->num_atoms : (pr.n_struct ? pr.n_struct : pr.h_idx[0].size())), cap));
+            if (pr.n_struct) CUDA_TRY(ps.d_com.alloc((size_t)p->B * pr.n_struct * 3));
+            else {
+                CUDA_TRY(ps.d_pair_list.alloc((size_t)p->B * rdf_list_stride(p, pr, first_cell)));
+                CUDA_TRY(ps.d_list_hdr.alloc((size_t)p->B * cap));
+                CUDA_TRY(ps.d_list_cursor.alloc(p->B));
+            }
+            CUDA_TRY(ps.d_frame_bins.alloc((size_t)p->B * (MDGPU_DIST_BINS + 1)));   // + one work counter per frame (k_rdf_pairs_v2)
+        } else if (pr.op == MDGPU_OP_CONTACT_COUNT) {
+            CUDA_TRY(ps.ref.alloc(p->B, (uint32_t)pr.h_idx[0].size(), cap));
+            CUDA_TRY(ps.d_frame_bins.alloc((size_t)p->B * (MDGPU_DIST_BINS + 1)));
+        } else if (pr.op == MDGPU_OP_SDF) {
+            CUDA_TRY(ps.d_sdf_xyzw.alloc((size_t)p->B * (pr.n_struct + 1) * pr.struct_size));
+            CUDA_TRY(ps.d_sdf_ref0.alloc((size_t)p->B * 20));
+            CUDA_TRY(ps.d_sdf_mats.alloc((size_t)p->B * pr.n_struct * 32));
+        } else if (pr.op == MDGPU_OP_DISTANCE_PAIR || ((pr.op == MDGPU_OP_DISTANCE_MIN || pr.op == MDGPU_OP_DISTANCE_MAX || (pr.op >= MDGPU_OP_COORD_X && pr.op <= MDGPU_OP_COORD_Z) || pr.op == MDGPU_OP_PLANE) && (!pr.h_goff[0].empty() || !pr.h_goff[1].empty()))) {
+            for (int k = 0; k < 2; ++k) if (!pr.h_goff[k].empty()) CUDA_TRY(ps.d_gpos[k].alloc((size_t)p->B * (pr.h_goff[k].size() - 1) * 3));
+            if (pr.op == MDGPU_OP_PLANE) CUDA_TRY(ps.d_sdf_xyzw.alloc((size_t)p->B * pr.h_idx[0].size()));   // the plane fit's xyzw scratch
+        } else if (pr.op == MDGPU_OP_WITHIN_COUNT) {
+            CUDA_TRY(ps.d_geom.alloc(p->B)); CUDA_TRY(ps.d_aabb.alloc((size_t)6 * p->B));
+            CUDA_TRY(ps.trg.alloc(p->B, (uint32_t)p->num_atoms, cap));
+            CUDA_TRY(ps.ref.alloc(p->B, (uint32_t)std::max<size_t>(pr.h_idx[0].size(), 1), cap));
+            CUDA_TRY(ps.d_flags.alloc((size_t)p->B * p->num_atoms));
+        } else if (pr.op == MDGPU_OP_POROSITY) {
+            CUDA_TRY(ps.d_poro_xyzr.alloc((size_t)PORO_FRAMES * pr.h_idx[0].size())); CUDA_TRY(ps.d_poro_hdr.alloc(PORO_FRAMES));
+            CUDA_TRY(ps.d_poro_grid.alloc((size_t)PORO_FRAMES * PORO_GRID_WORDS)); CUDA_TRY(ps.d_poro_count.alloc(PORO_FRAMES));
+            CUDA_TRY(cudaMemset(ps.d_poro_grid.get(), 0, ps.d_poro_grid.bytes()));
+            CUDA_TRY(cudaMemset(ps.d_poro_count.get(), 0, ps.d_poro_count.bytes()));
+        } else if (pr.op == MDGPU_OP_RMSD) {
+            CUDA_TRY(ps.d_sdf_xyzw.alloc((size_t)p->B * 2 * pr.h_idx[0].size()));   // [B][initial, current][atoms]
+        } else if (pr.op == MDGPU_OP_PLANE || pr.op == MDGPU_OP_SHAPE_WEIGHTS) {
+            CUDA_TRY(ps.d_sdf_xyzw.alloc((size_t)p->B * pr.h_idx[0].size()));
+        } else if (pr.op >= MDGPU_OP_DENSITY_X && pr.op <= MDGPU_OP_DENSITY_Z) {
+            CUDA_TRY(ps.d_frame_bins64.alloc((size_t)p->B * MDGPU_DIST_BINS));
+        } else if (pr.com_mask) {
+            if (!pr.n_struct) CUDA_TRY(ps.d_argpos.alloc((size_t)p->B * 12));
+            for (int k = 0; k < 4; ++k) if (!pr.h_aoff[k].empty()) CUDA_TRY(ps.d_parts[k].alloc((size_t)p->B * (pr.h_aoff[k].size() - 1)));
+        }
+    }
+    return 0;
+}
+
+// slot set-up (lazy: needs the first frame's cell for the default cell capacity). All or nothing: the slots and each slot's host staging
+// become the plan's only once all their allocations have succeeded; after a failure the owners free what was built and the next call
+// builds again.
 static int ensure_slots(mdgpu_plan* p, const mdgpu_unitcell_t* first_cell, bool need_host_staging) {
     std::lock_guard<std::mutex> guard(p->slot_mutex);   // concurrent callers: the first one builds the slots
     if (p->slots.empty()) {
@@ -817,84 +905,17 @@ static int ensure_slots(mdgpu_plan* p, const mdgpu_unitcell_t* first_cell, bool 
                 need = std::max<uint64_t>(need, 2ull * std::max<uint64_t>(g.num_cells, g.num_home) + 2);
             }
             cap = (uint32_t)std::min<uint64_t>(need, 1u << 26);
-            p->cell_cap = cap;
         }
-        p->slots.resize(p->S);
-        for (auto& s : p->slots) {
-            CUDA_TRY(cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking));
-            CUDA_TRY(cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming));
-            CUDA_TRY(cudaEventCreateWithFlags(&s.copied, cudaEventDisableTiming));
-            CUDA_TRY(cudaMallocHost((void**)&s.h_err, sizeof(int))); *s.h_err = 0;
-            CUDA_TRY(dalloc(&s.d_cells, p->B));
-            CUDA_TRY(cudaMallocHost((void**)&s.h_cells, sizeof(mdgpu_unitcell_t) * p->B));
-            CUDA_TRY(dalloc(&s.d_err, 1)); CUDA_TRY(cudaMemset(s.d_err, 0, sizeof(int)));
-            s.ps.resize(p->props.size());
-            for (size_t i = 0; i < p->props.size(); ++i) {
-                Prop& pr = p->props[i]; PropScratch& ps = s.ps[i];
-                for (int k = 0; k < 4; ++k) if (pr.dyn[k].on) {   // the within() query of a dynamic argument: system-wide lists + marks + per-frame index list
-                    auto& w = ps.dynw[k];
-                    CUDA_TRY(dalloc(&w.d_geom, p->B)); CUDA_TRY(dalloc(&w.d_aabb, (size_t)6 * p->B));
-                    int rc = alloc_cell_list(w.trg, p->B, (uint32_t)p->num_atoms, cap); if (rc) return rc;
-                    rc = alloc_cell_list(w.ref, p->B, (uint32_t)std::max<size_t>(pr.h_idx[k].size(), 1), cap); if (rc) return rc;
-                    CUDA_TRY(dalloc(&w.d_flags, (size_t)p->B * p->num_atoms));
-                    CUDA_TRY(dalloc(&w.d_idx, (size_t)p->B * p->num_atoms)); CUDA_TRY(dalloc(&w.d_n, p->B));
-                }
-                if (pr.needs_cells() && pr.share_trg < 0) {
-                    CUDA_TRY(dalloc(&ps.d_geom, p->B)); CUDA_TRY(dalloc(&ps.d_aabb, (size_t)6 * p->B));
-                    int rc = alloc_cell_list(ps.trg, p->B, (uint32_t)(pr.dyn[1].on ? p->num_atoms : (pr.trg_groups ? pr.trg_groups : pr.h_idx[1].size())), cap); if (rc) return rc;
-                    if (pr.trg_groups) CUDA_TRY(dalloc(&ps.d_gpos[1], (size_t)p->B * pr.trg_groups * 3));
-                }
-                if (pr.op == MDGPU_OP_RDF) {
-                    int rc = alloc_cell_list(ps.ref, p->B, (uint32_t)(pr.dyn[0].on ? p->num_atoms : (pr.n_struct ? pr.n_struct : pr.h_idx[0].size())), cap); if (rc) return rc;
-                    if (pr.n_struct) CUDA_TRY(dalloc(&ps.d_com, (size_t)p->B * pr.n_struct * 3));
-                    else {   // candidate lists of the packed pair kernel: every target appears in at most (2n+1)^3 home cells' lists
-                        FrameGeom g; host_frame_geom(&g, first_cell, pr.cutoff_max, pr.cutoff_max, nullptr, 0xffffffffu);
-                        size_t nn = (size_t)(2 * std::max(g.ncell[0], 1) + 1) * (2 * std::max(g.ncell[1], 1) + 1) * (2 * std::max(g.ncell[2], 1) + 1);
-                        if (g.valid <= 0 || (first_cell->flags & MDGPU_CELL_PBC_ALL) != MDGPU_CELL_PBC_ALL) nn = 125;   // grid from the data (AABB fit): size for the widest reach the reference allows
-                        // a dynamic target set is sized for a quarter of the system; frames that select more are finished by the overflow pass
-                        ps.list_stride = std::min<size_t>(nn, 125) * (pr.dyn[1].on ? std::max<size_t>(p->num_atoms / 4, 1024) : pr.h_idx[1].size()) + 1024;
-                        CUDA_TRY(dalloc(&ps.d_pair_list, (size_t)p->B * ps.list_stride));
-                        CUDA_TRY(dalloc(&ps.d_list_hdr, (size_t)p->B * cap));
-                        CUDA_TRY(dalloc(&ps.d_list_cursor, p->B));
-                    }
-                    CUDA_TRY(dalloc(&ps.d_frame_bins, (size_t)p->B * (MDGPU_DIST_BINS + 1)));   // + one work counter per frame (k_rdf_pairs_v2)
-                } else if (pr.op == MDGPU_OP_CONTACT_COUNT) {
-                    int rc = alloc_cell_list(ps.ref, p->B, (uint32_t)pr.h_idx[0].size(), cap); if (rc) return rc;
-                    CUDA_TRY(dalloc(&ps.d_frame_bins, (size_t)p->B * (MDGPU_DIST_BINS + 1)));
-                } else if (pr.op == MDGPU_OP_SDF) {
-                    CUDA_TRY(dalloc(&ps.d_sdf_xyzw, (size_t)p->B * (pr.n_struct + 1) * pr.struct_size));
-                    CUDA_TRY(dalloc(&ps.d_sdf_ref0, (size_t)p->B * 20));
-                    CUDA_TRY(dalloc(&ps.d_sdf_mats, (size_t)p->B * pr.n_struct * 32));
-                } else if (pr.op == MDGPU_OP_DISTANCE_PAIR || ((pr.op == MDGPU_OP_DISTANCE_MIN || pr.op == MDGPU_OP_DISTANCE_MAX || (pr.op >= MDGPU_OP_COORD_X && pr.op <= MDGPU_OP_COORD_Z) || pr.op == MDGPU_OP_PLANE) && (!pr.h_goff[0].empty() || !pr.h_goff[1].empty()))) {
-                    for (int k = 0; k < 2; ++k) if (!pr.h_goff[k].empty()) CUDA_TRY(dalloc(&ps.d_gpos[k], (size_t)p->B * (pr.h_goff[k].size() - 1) * 3));
-                    if (pr.op == MDGPU_OP_PLANE) CUDA_TRY(dalloc(&ps.d_sdf_xyzw, (size_t)p->B * pr.h_idx[0].size()));   // the plane fit's xyzw scratch
-                } else if (pr.op == MDGPU_OP_WITHIN_COUNT) {
-                    CUDA_TRY(dalloc(&ps.d_geom, p->B)); CUDA_TRY(dalloc(&ps.d_aabb, (size_t)6 * p->B));
-                    int rc = alloc_cell_list(ps.trg, p->B, (uint32_t)p->num_atoms, cap); if (rc) return rc;
-                    rc = alloc_cell_list(ps.ref, p->B, (uint32_t)std::max<size_t>(pr.h_idx[0].size(), 1), cap); if (rc) return rc;
-                    CUDA_TRY(dalloc(&ps.d_flags, (size_t)p->B * p->num_atoms));
-                } else if (pr.op == MDGPU_OP_POROSITY) {
-                    CUDA_TRY(dalloc(&ps.d_poro_xyzr, (size_t)PORO_FRAMES * pr.h_idx[0].size())); CUDA_TRY(dalloc(&ps.d_poro_hdr, PORO_FRAMES));
-                    CUDA_TRY(dalloc(&ps.d_poro_grid, (size_t)PORO_FRAMES * PORO_GRID_WORDS)); CUDA_TRY(dalloc(&ps.d_poro_count, PORO_FRAMES));
-                    CUDA_TRY(cudaMemset(ps.d_poro_grid, 0, sizeof(unsigned long long) * PORO_FRAMES * PORO_GRID_WORDS));
-                    CUDA_TRY(cudaMemset(ps.d_poro_count, 0, sizeof(unsigned long long) * PORO_FRAMES));
-                } else if (pr.op == MDGPU_OP_RMSD) {
-                    CUDA_TRY(dalloc(&ps.d_sdf_xyzw, (size_t)p->B * 2 * pr.h_idx[0].size()));   // [B][initial, current][atoms]
-                } else if (pr.op == MDGPU_OP_PLANE || pr.op == MDGPU_OP_SHAPE_WEIGHTS) {
-                    CUDA_TRY(dalloc(&ps.d_sdf_xyzw, (size_t)p->B * pr.h_idx[0].size()));
-                } else if (pr.op >= MDGPU_OP_DENSITY_X && pr.op <= MDGPU_OP_DENSITY_Z) {
-                    CUDA_TRY(dalloc(&ps.d_frame_bins64, (size_t)p->B * MDGPU_DIST_BINS));
-                } else if (pr.com_mask) {
-                    if (!pr.n_struct) CUDA_TRY(dalloc(&ps.d_argpos, (size_t)p->B * 12));
-                    for (int k = 0; k < 4; ++k) if (!pr.h_aoff[k].empty()) CUDA_TRY(dalloc(&ps.d_parts[k], (size_t)p->B * (pr.h_aoff[k].size() - 1)));
-                }
-            }
-        }
+        std::vector<Slot> slots(p->S);
+        for (auto& s : slots) { const int rc = build_slot(p, s, first_cell, cap); if (rc) return rc; }
+        p->slots = std::move(slots); p->cell_cap = cap;
     }
-    if (need_host_staging) for (auto& s : p->slots) if (!s.d_frames) {   // host ingest staging, in the ingest (compact or full) atom space
-        const size_t AS = p->compact ? p->axis_stride_c : p->axis_stride;
-        CUDA_TRY(dalloc(&s.d_frames, (size_t)p->B * 3 * AS));
-        CUDA_TRY(cudaMallocHost((void**)&s.h_frames, sizeof(float) * (size_t)p->B * 3 * AS));
+    if (need_host_staging) for (auto& s : p->slots) if (!s.d_frames.get()) {   // host ingest staging, in the ingest (compact or full) atom space
+        const size_t n = (size_t)p->B * 3 * (p->compact ? p->axis_stride_c : p->axis_stride);
+        DevBuf<float> d; PinnedBuf<float> h;
+        CUDA_TRY(d.alloc(n));
+        CUDA_TRY(h.alloc(n));
+        s.d_frames = std::move(d); s.h_frames = std::move(h);
     }
     return 0;
 }
@@ -907,9 +928,9 @@ static int ensure_slots(mdgpu_plan* p, const mdgpu_unitcell_t* first_cell, bool 
 static void arg_position(Prop& pr, PropScratch& ps, int k, const BatchFrames& fr, Slot& s, int32_t* const* didx, const float* dmass, DynSel dsel) {
     if (!pr.h_aoff[k].empty()) {
         const uint32_t n = (uint32_t)pr.h_aoff[k].size() - 1u;
-        launch_arg_com_parts(fr, s.d_cells, didx[k], pr.d_aoff[k], n, dmass, ps.d_parts[k], s.stream);
-        launch_arg_combine(ps.d_parts[k], n, s.d_cells, ps.d_argpos, k, (int)fr.count, s.stream);
-    } else launch_arg_com(fr, s.d_cells, didx[k], (uint32_t)pr.h_idx[k].size(), dmass, ps.d_argpos, k, s.stream, dsel);
+        launch_arg_com_parts(fr, s.d_cells.get(), didx[k], pr.d_aoff[k].get(), n, dmass, ps.d_parts[k].get(), s.stream);
+        launch_arg_combine(ps.d_parts[k].get(), n, s.d_cells.get(), ps.d_argpos.get(), k, (int)fr.count, s.stream);
+    } else launch_arg_com(fr, s.d_cells.get(), didx[k], (uint32_t)pr.h_idx[k].size(), dmass, ps.d_argpos.get(), k, s.stream, dsel);
 }
 
 static int enqueue_batch(mdgpu_plan* p, Slot& s, const BatchFrames& fr, uint32_t frame0, bool c) {
@@ -919,12 +940,12 @@ static int enqueue_batch(mdgpu_plan* p, Slot& s, const BatchFrames& fr, uint32_t
     bool tri = (s.h_cells[0].flags & MDGPU_CELL_TRICLINIC) != 0;
     for (int i = 1; i < B; ++i) if (((s.h_cells[i].flags & MDGPU_CELL_TRICLINIC) != 0) != tri)
         return fail(MDGPU_ERR_UNSUPPORTED, "frames %u..%u mix orthorhombic and triclinic unit cells inside one batch", frame0, frame0 + B - 1);
-    CUDA_TRY(cudaMemcpyAsync(s.d_cells, s.h_cells, sizeof(mdgpu_unitcell_t) * B, cudaMemcpyHostToDevice, s.stream));
+    CUDA_TRY(cudaMemcpyAsync(s.d_cells.get(), s.h_cells.get(), sizeof(mdgpu_unitcell_t) * B, cudaMemcpyHostToDevice, s.stream));
     bool all_pbc = true; for (int i = 0; i < B; ++i) all_pbc = all_pbc && ((s.h_cells[i].flags & MDGPU_CELL_PBC_ALL) == MDGPU_CELL_PBC_ALL);
     for (size_t i = 0; i < p->props.size(); ++i) {
         Prop& pr = p->props[i]; PropScratch& ps = s.ps[i];
-        int32_t* const* didx = c ? pr.d_idx_c : pr.d_idx;
-        const float* dmass = c ? p->d_mass_c : p->d_mass; const float* dinit = c ? p->d_init_c : p->d_init; const size_t init_as = c ? p->axis_stride_c : p->axis_stride;
+        int32_t* didx[4]; for (int k = 0; k < 4; ++k) didx[k] = (c ? pr.d_idx_c[k] : pr.d_idx[k]).get();
+        const float* dmass = c ? p->d_mass_c.get() : p->d_mass.get(); const float* dinit = c ? p->d_init_c.get() : p->d_init.get(); const size_t init_as = c ? p->axis_stride_c : p->axis_stride;
         const PropScratch& cs = (pr.share_trg >= 0) ? s.ps[pr.share_trg] : ps;   // owner of the target cell list + geometry
         DynSel dsel[4];
         for (int k = 0; k < 4; ++k) {   // dynamic arguments first: within([min:]max, idx[k]) [and mask] of every frame of the batch -> ascending per-frame lists
@@ -932,92 +953,87 @@ static int enqueue_batch(mdgpu_plan* p, Slot& s, const BatchFrames& fr, uint32_t
             if (!pr.dyn[k].on) continue;
             auto& w = ps.dynw[k];
             const float* waabb = nullptr;
-            if (!all_pbc) { launch_aabb(fr, nullptr, (uint32_t)p->num_atoms, w.d_aabb, s.stream); waabb = w.d_aabb; }   // every atom of the system (get_spatial_acc :734)
-            launch_geom(s.d_cells, waabb, w.d_geom, within_cell_ext(pr.dyn[k].rmax), (double)pr.dyn[k].rmax, p->cell_cap, B, s.d_err, s.stream);
-            launch_cell_list(0, fr, nullptr, nullptr, (uint32_t)p->num_atoms, w.d_geom, w.trg, 0, s.stream);
-            launch_cell_list(1, fr, didx[k], nullptr, (uint32_t)pr.h_idx[k].size(), w.d_geom, w.ref, 0, s.stream);
+            if (!all_pbc) { launch_aabb(fr, nullptr, (uint32_t)p->num_atoms, w.d_aabb.get(), s.stream); waabb = w.d_aabb.get(); }   // every atom of the system (get_spatial_acc :734)
+            launch_geom(s.d_cells.get(), waabb, w.d_geom.get(), within_cell_ext(pr.dyn[k].rmax), (double)pr.dyn[k].rmax, p->cell_cap, B, s.d_err.get(), s.stream);
+            launch_cell_list(0, fr, nullptr, nullptr, (uint32_t)p->num_atoms, w.d_geom.get(), w.trg.cl, 0, s.stream);
+            launch_cell_list(1, fr, didx[k], nullptr, (uint32_t)pr.h_idx[k].size(), w.d_geom.get(), w.ref.cl, 0, s.stream);
             WithinArgs wa{};
-            wa.geom = w.d_geom; wa.trg = w.trg; wa.ref = w.ref; wa.sel = didx[k]; wa.n_sel = (uint32_t)pr.h_idx[k].size();
-            wa.num_atoms = (uint32_t)p->num_atoms; wa.flags = w.d_flags; wa.out = nullptr; wa.frame0 = frame0; wa.min_r2 = pr.dyn[k].rmin * pr.dyn[k].rmin; wa.and_mask = pr.dyn[k].d_and_mask;
-            launch_within_list(wa, B, tri, p->sm_count, w.d_idx, w.d_n, s.stream);
-            dsel[k] = DynSel{ w.d_idx, w.d_n, (uint32_t)p->num_atoms };
+            wa.geom = w.d_geom.get(); wa.trg = w.trg.cl; wa.ref = w.ref.cl; wa.sel = didx[k]; wa.n_sel = (uint32_t)pr.h_idx[k].size();
+            wa.num_atoms = (uint32_t)p->num_atoms; wa.flags = w.d_flags.get(); wa.out = nullptr; wa.frame0 = frame0; wa.min_r2 = pr.dyn[k].rmin * pr.dyn[k].rmin; wa.and_mask = pr.dyn[k].d_and_mask.get();
+            launch_within_list(wa, B, tri, p->sm_count, w.d_idx.get(), w.d_n.get(), s.stream);
+            dsel[k] = DynSel{ w.d_idx.get(), w.d_n.get(), (uint32_t)p->num_atoms };
         }
         if (pr.needs_cells() && pr.share_trg < 0) {
             const float* aabb = nullptr;
             if (pr.trg_groups) {   // the target points are the groups' centres of mass: an AoS stream, j = position index (compute_rdf :5299-5301)
-                launch_group_com(fr, didx[1], pr.d_goff[1], (uint32_t)pr.trg_groups, dmass, ps.d_gpos[1], s.stream);
-                if (!all_pbc) { launch_aabb(fr, nullptr, (uint32_t)pr.trg_groups, ps.d_aabb, s.stream, DynSel{ nullptr, nullptr, 0 }, ps.d_gpos[1]); aabb = ps.d_aabb; }
-                launch_geom(s.d_cells, aabb, ps.d_geom, (double)pr.cutoff_max, (double)pr.cutoff_max, p->cell_cap, B, s.d_err, s.stream);
-                launch_cell_list(0, fr, nullptr, ps.d_gpos[1], (uint32_t)pr.trg_groups, ps.d_geom, ps.trg, 0, s.stream);
+                launch_group_com(fr, didx[1], pr.d_goff[1].get(), (uint32_t)pr.trg_groups, dmass, ps.d_gpos[1].get(), s.stream);
+                if (!all_pbc) { launch_aabb(fr, nullptr, (uint32_t)pr.trg_groups, ps.d_aabb.get(), s.stream, DynSel{ nullptr, nullptr, 0 }, ps.d_gpos[1].get()); aabb = ps.d_aabb.get(); }
+                launch_geom(s.d_cells.get(), aabb, ps.d_geom.get(), (double)pr.cutoff_max, (double)pr.cutoff_max, p->cell_cap, B, s.d_err.get(), s.stream);
+                launch_cell_list(0, fr, nullptr, ps.d_gpos[1].get(), (uint32_t)pr.trg_groups, ps.d_geom.get(), ps.trg.cl, 0, s.stream);
             } else {
-            if (!all_pbc) { launch_aabb(fr, didx[1], (uint32_t)pr.h_idx[1].size(), ps.d_aabb, s.stream, dsel[1]); aabb = ps.d_aabb; }
-            launch_geom(s.d_cells, aabb, ps.d_geom, (double)pr.cutoff_max, (double)pr.cutoff_max, p->cell_cap, B, s.d_err, s.stream);
-            launch_cell_list(0, fr, didx[1], nullptr, (uint32_t)pr.h_idx[1].size(), ps.d_geom, ps.trg, 0, s.stream, dsel[1]);
+            if (!all_pbc) { launch_aabb(fr, didx[1], (uint32_t)pr.h_idx[1].size(), ps.d_aabb.get(), s.stream, dsel[1]); aabb = ps.d_aabb.get(); }
+            launch_geom(s.d_cells.get(), aabb, ps.d_geom.get(), (double)pr.cutoff_max, (double)pr.cutoff_max, p->cell_cap, B, s.d_err.get(), s.stream);
+            launch_cell_list(0, fr, didx[1], nullptr, (uint32_t)pr.h_idx[1].size(), ps.d_geom.get(), ps.trg.cl, 0, s.stream, dsel[1]);
             }
         }
         switch (pr.op) {
         case MDGPU_OP_RDF: {
             if (pr.dyn[0].on) {   // references = the frame's dynamic selection (coordinate_extract on a single bitfield: ascending atoms; compute_rdf :5281-5290)
-                launch_cell_list(1, fr, nullptr, nullptr, 0, cs.d_geom, ps.ref, 0, s.stream, dsel[0]);
+                launch_cell_list(1, fr, nullptr, nullptr, 0, cs.d_geom.get(), ps.ref.cl, 0, s.stream, dsel[0]);
             } else if (pr.n_struct) {
-                launch_group_com(fr, didx[0], pr.d_soff, (uint32_t)pr.n_struct, dmass, ps.d_com, s.stream);
-                launch_cell_list(1, fr, nullptr, ps.d_com, (uint32_t)pr.n_struct, cs.d_geom, ps.ref, 0, s.stream);   // AoS stream: i = position index (:1721)
+                launch_group_com(fr, didx[0], pr.d_soff.get(), (uint32_t)pr.n_struct, dmass, ps.d_com.get(), s.stream);
+                launch_cell_list(1, fr, nullptr, ps.d_com.get(), (uint32_t)pr.n_struct, cs.d_geom.get(), ps.ref.cl, 0, s.stream);   // AoS stream: i = position index (:1721)
             } else {
-                launch_cell_list(1, fr, didx[0], nullptr, (uint32_t)pr.h_idx[0].size(), cs.d_geom, ps.ref, 0, s.stream);
+                launch_cell_list(1, fr, didx[0], nullptr, (uint32_t)pr.h_idx[0].size(), cs.d_geom.get(), ps.ref.cl, 0, s.stream);
             }
-            if (!pr.n_struct) {   // candidate lists: the neighbour reach follows the frame's cell (an NPT or sheared cell can cross from 27 to 125 offsets)
-                size_t nn_max = 0;
+            if (!pr.n_struct) {   // candidate lists: the neighbour reach follows the frame's cell
+                size_t need = 0;
                 for (int i = 0; i < B; ++i) {
                     if (!ps.nn_valid || memcmp(&ps.nn_cell, &s.h_cells[i], sizeof(mdgpu_unitcell_t)) != 0) {   // constant-cell trajectories: one evaluation
-                        FrameGeom g; host_frame_geom(&g, &s.h_cells[i], pr.cutoff_max, pr.cutoff_max, nullptr, 0xffffffffu);
-                        size_t nn = (size_t)(2 * std::max(g.ncell[0], 1) + 1) * (2 * std::max(g.ncell[1], 1) + 1) * (2 * std::max(g.ncell[2], 1) + 1);
-                        if (g.valid <= 0 || (s.h_cells[i].flags & MDGPU_CELL_PBC_ALL) != MDGPU_CELL_PBC_ALL) nn = 125;
-                        ps.nn_cell = s.h_cells[i]; ps.nn_of_cell = std::min<size_t>(nn, 125); ps.nn_valid = true;
+                        ps.nn_cell = s.h_cells[i]; ps.nn_stride = rdf_list_stride(p, pr, &s.h_cells[i]); ps.nn_valid = true;
                     }
-                    nn_max = std::max(nn_max, ps.nn_of_cell);
+                    need = std::max(need, ps.nn_stride);
                 }
-                const size_t need = nn_max * (pr.dyn[1].on ? std::max<size_t>(p->num_atoms / 4, 1024) : pr.h_idx[1].size()) + 1024;
-                if (need > ps.list_stride) {   // the slot was retired before this batch: its buffers are idle
+                if ((size_t)p->B * need > ps.d_pair_list.size()) {   // the slot was retired before this batch: its buffers are idle
                     CUDA_TRY(cudaStreamSynchronize(s.stream));
-                    cudaFree(ps.d_pair_list); ps.d_pair_list = nullptr; ps.list_stride = need;
-                    CUDA_TRY(dalloc(&ps.d_pair_list, (size_t)p->B * ps.list_stride));
+                    CUDA_TRY(ps.d_pair_list.alloc((size_t)p->B * need));   // on failure the list is empty and the next batch tries again
                 }
             }
             RdfArgs a{};
-            a.geom = cs.d_geom; a.trg = cs.trg; a.ref = ps.ref;
+            a.geom = cs.d_geom.get(); a.trg = cs.trg.cl; a.ref = ps.ref.cl;
             a.inv_cutoff_range = 1.0f / (pr.cutoff_max - pr.cutoff_min);                 // before the clamp (compute_rdf :5264)
             a.min_cutoff = pr.cutoff_min > 1e-3f ? pr.cutoff_min : 1e-3f;                 // :5269
             a.min_r2 = a.min_cutoff * a.min_cutoff;                                       // rdf_cb :5233
-            a.frame_bins = ps.d_frame_bins; a.frame0 = frame0;
-            a.pair_list = ps.d_pair_list; a.list_hdr = ps.d_list_hdr; a.list_cursor = ps.d_list_cursor; a.list_stride = ps.list_stride; a.hdr_stride = p->cell_cap; a.err = s.d_err;
-            a.excl_off = pr.n_struct ? pr.d_soff : nullptr; a.excl_idx = pr.n_struct ? didx[0] : nullptr;   // md_bitfield_test_bit(&masks[i], j) :5252
+            a.frame_bins = ps.d_frame_bins.get(); a.frame0 = frame0;
+            a.pair_list = ps.d_pair_list.get(); a.list_hdr = ps.d_list_hdr.get(); a.list_cursor = ps.d_list_cursor.get(); a.list_stride = ps.d_pair_list.size() / p->B; a.hdr_stride = p->cell_cap; a.err = s.d_err.get();
+            a.excl_off = pr.n_struct ? pr.d_soff.get() : nullptr; a.excl_idx = pr.n_struct ? didx[0] : nullptr;   // md_bitfield_test_bit(&masks[i], j) :5252
             a.symmetric = (!pr.n_struct && !pr.trg_groups && !pr.dyn[0].on && !pr.dyn[1].on && pr.h_idx[0] == pr.h_idx[1]) ? 1 : 0;   // same selection on both sides: unshifted pairs are evaluated once, counted twice
-            a.acc = pr.d_acc; a.frame_total = pr.d_frame_total; a.frame_min = pr.d_frame_min; a.frame_max = pr.d_frame_max; a.keep = pr.d_keep;
-            a.counters = p->timing ? p->d_counters : nullptr;
+            a.acc = pr.d_acc.get(); a.frame_total = pr.d_frame_total.get(); a.frame_min = pr.d_frame_min.get(); a.frame_max = pr.d_frame_max.get(); a.keep = pr.d_keep.get();
+            a.counters = p->timing ? p->d_counters.get() : nullptr;
             cudaEvent_t ev4[4] = { nullptr, nullptr, nullptr, nullptr };   // before cull, after cull, before pairs, after pairs
             if (p->timing) for (auto& e : ev4) cudaEventCreate(&e);
             launch_rdf(a, B, tri, (int)p->rdf_variant, p->sm_count, s.stream, p->timing ? ev4 : nullptr);
             if (p->timing) { p->timed.push_back(TimedLaunch{ ev4[0], ev4[1], 3 }); p->timed.push_back(TimedLaunch{ ev4[2], ev4[3], 0 }); }
             break; }
         case MDGPU_OP_CONTACT_COUNT: {   // external points = the atoms of all sets (tag: position in the list), internal = B (md_script_functions.inl:2808-2846)
-            launch_cell_list(1, fr, didx[0], nullptr, (uint32_t)pr.h_idx[0].size(), cs.d_geom, ps.ref, 1, s.stream);
+            launch_cell_list(1, fr, didx[0], nullptr, (uint32_t)pr.h_idx[0].size(), cs.d_geom.get(), ps.ref.cl, 1, s.stream);
             RdfArgs a{};
-            a.geom = cs.d_geom; a.trg = cs.trg; a.ref = ps.ref;
+            a.geom = cs.d_geom.get(); a.trg = cs.trg.cl; a.ref = ps.ref.cl;
             a.inv_cutoff_range = 1.0f; a.min_cutoff = 0.0f; a.min_r2 = 0.0f;
-            a.frame_bins = ps.d_frame_bins; a.frame0 = frame0; a.err = s.d_err;
-            a.excl_off = pr.d_goff[1]; a.excl_idx = didx[2]; a.ref_set = pr.d_set_of; a.count_mode = 1;
+            a.frame_bins = ps.d_frame_bins.get(); a.frame0 = frame0; a.err = s.d_err.get();
+            a.excl_off = pr.d_goff[1].get(); a.excl_idx = didx[2]; a.ref_set = pr.d_set_of.get(); a.count_mode = 1;
             launch_rdf(a, B, tri, 1, p->sm_count, s.stream, nullptr);
-            launch_contact_rows(ps.d_frame_bins, (uint32_t)pr.n_struct, pr.d_temporal, frame0, B, s.stream);
+            launch_contact_rows(ps.d_frame_bins.get(), (uint32_t)pr.n_struct, pr.d_temporal.get(), frame0, B, s.stream);
             break; }
         case MDGPU_OP_SDF: {
             if (!p->have_init) return fail(MDGPU_ERR_INVALID_ARG, "sdf '%s' needs the initial frame (mdgpu_plan_set_initial_frame)", pr.name.c_str());
             SdfArgs a{};
-            a.geom = cs.d_geom; a.trg = cs.trg; a.frames = fr; a.cells = s.d_cells;
+            a.geom = cs.d_geom.get(); a.trg = cs.trg.cl; a.frames = fr; a.cells = s.d_cells.get();
             a.init_xyz = dinit; a.init_axis_stride = init_as; a.mass = dmass;
             a.struct_idx = didx[0]; a.n_struct = (uint32_t)pr.n_struct; a.struct_size = (uint32_t)pr.struct_size;
-            a.unwrap_pairs = pr.d_unwrap; a.n_unwrap = pr.n_unwrap; a.cutoff = pr.cutoff_max;
-            a.scratch_xyzw = ps.d_sdf_xyzw; a.ref0 = ps.d_sdf_ref0; a.matrices = ps.d_sdf_mats;
-            a.vol = pr.d_vol; a.frame_total = pr.d_frame_total; a.frame0 = frame0;
+            a.unwrap_pairs = pr.d_unwrap.get(); a.n_unwrap = pr.n_unwrap; a.cutoff = pr.cutoff_max;
+            a.scratch_xyzw = ps.d_sdf_xyzw.get(); a.ref0 = ps.d_sdf_ref0.get(); a.matrices = ps.d_sdf_mats.get();
+            a.vol = pr.d_vol.get(); a.frame_total = pr.d_frame_total.get(); a.frame0 = frame0;
             TimedLaunch tl{};
             if (p->timing) { cudaEventCreate(&tl.a); cudaEventCreate(&tl.b); cudaEventRecord(tl.a, s.stream); }
             launch_sdf(a, B, tri, s.stream);
@@ -1028,7 +1044,7 @@ static int enqueue_batch(mdgpu_plan* p, Slot& s, const BatchFrames& fr, uint32_t
             DensityArgs a{};
             a.frames = fr; a.idx = didx[0]; a.n = (uint32_t)pr.h_idx[0].size(); a.mass = dmass; a.axis = (int)pr.op - MDGPU_OP_DENSITY_X; a.dyn = dsel[0];
             a.rc = pr.rc; a.re = pr.re; a.inv_ext = pr.inv_ext; a.min_point = pr.min_point;
-            a.acc = pr.d_acc; a.frame_bins = ps.d_frame_bins64; a.frame_min = pr.d_frame_min64; a.frame_max = pr.d_frame_max64; a.keep = pr.d_keep64; a.frame0 = frame0;
+            a.acc = pr.d_acc.get(); a.frame_bins = ps.d_frame_bins64.get(); a.frame_min = pr.d_frame_min64.get(); a.frame_max = pr.d_frame_max64.get(); a.keep = pr.d_keep64.get(); a.frame0 = frame0;
             TimedLaunch tl{};
             if (p->timing) { cudaEventCreate(&tl.a); cudaEventCreate(&tl.b); cudaEventRecord(tl.a, s.stream); }
             launch_density(a, B, s.stream);
@@ -1036,73 +1052,73 @@ static int enqueue_batch(mdgpu_plan* p, Slot& s, const BatchFrames& fr, uint32_t
             break; }
         case MDGPU_OP_WITHIN_COUNT: {
             const float* aabb = nullptr;
-            if (!all_pbc) { launch_aabb(fr, nullptr, (uint32_t)p->num_atoms, ps.d_aabb, s.stream); aabb = ps.d_aabb; }   // every atom of the system
-            launch_geom(s.d_cells, aabb, ps.d_geom, within_cell_ext(pr.cutoff_max), (double)pr.cutoff_max, p->cell_cap, B, s.d_err, s.stream);
-            launch_cell_list(0, fr, nullptr, nullptr, (uint32_t)p->num_atoms, ps.d_geom, ps.trg, 0, s.stream);
-            launch_cell_list(1, fr, didx[0], nullptr, (uint32_t)pr.h_idx[0].size(), ps.d_geom, ps.ref, 0, s.stream);
+            if (!all_pbc) { launch_aabb(fr, nullptr, (uint32_t)p->num_atoms, ps.d_aabb.get(), s.stream); aabb = ps.d_aabb.get(); }   // every atom of the system
+            launch_geom(s.d_cells.get(), aabb, ps.d_geom.get(), within_cell_ext(pr.cutoff_max), (double)pr.cutoff_max, p->cell_cap, B, s.d_err.get(), s.stream);
+            launch_cell_list(0, fr, nullptr, nullptr, (uint32_t)p->num_atoms, ps.d_geom.get(), ps.trg.cl, 0, s.stream);
+            launch_cell_list(1, fr, didx[0], nullptr, (uint32_t)pr.h_idx[0].size(), ps.d_geom.get(), ps.ref.cl, 0, s.stream);
             WithinArgs a{};
-            a.geom = ps.d_geom; a.trg = ps.trg; a.ref = ps.ref; a.sel = didx[0]; a.n_sel = (uint32_t)pr.h_idx[0].size();
-            a.num_atoms = (uint32_t)p->num_atoms; a.flags = ps.d_flags; a.out = pr.d_temporal; a.frame0 = frame0; a.min_r2 = pr.cutoff_min * pr.cutoff_min; a.and_mask = pr.d_and_mask;   // :2641
+            a.geom = ps.d_geom.get(); a.trg = ps.trg.cl; a.ref = ps.ref.cl; a.sel = didx[0]; a.n_sel = (uint32_t)pr.h_idx[0].size();
+            a.num_atoms = (uint32_t)p->num_atoms; a.flags = ps.d_flags.get(); a.out = pr.d_temporal.get(); a.frame0 = frame0; a.min_r2 = pr.cutoff_min * pr.cutoff_min; a.and_mask = pr.d_and_mask.get();   // :2641
             launch_within_count(a, B, tri, p->sm_count, s.stream);
             break; }
         case MDGPU_OP_COM: {
             TemporalArgs a{};
-            a.frames = fr; a.cells = s.d_cells; a.op = (int)pr.op; a.out = pr.d_temporal; a.frame0 = frame0;
-            a.atom[0] = c ? pr.first_c[0] : pr.h_idx[0][0]; a.pos = ps.d_argpos; a.com_mask = pr.com_mask;
+            a.frames = fr; a.cells = s.d_cells.get(); a.op = (int)pr.op; a.out = pr.d_temporal.get(); a.frame0 = frame0;
+            a.atom[0] = c ? pr.first_c[0] : pr.h_idx[0][0]; a.pos = ps.d_argpos.get(); a.com_mask = pr.com_mask;
             if (pr.com_mask & 1u) arg_position(pr, ps, 0, fr, s, didx, dmass, dsel[0]);
             launch_com_rows(a, B, s.stream);
             break; }
         case MDGPU_OP_COORD_X: case MDGPU_OP_COORD_Y: case MDGPU_OP_COORD_Z:
             if (!pr.h_goff[0].empty()) {
                 const uint32_t n = (uint32_t)pr.h_goff[0].size() - 1;
-                launch_group_com(fr, didx[0], pr.d_goff[0], n, dmass, ps.d_gpos[0], s.stream);
-                launch_coord_rows_pos(ps.d_gpos[0], n, (int)pr.op - MDGPU_OP_COORD_X, pr.d_temporal, frame0, B, s.stream);
+                launch_group_com(fr, didx[0], pr.d_goff[0].get(), n, dmass, ps.d_gpos[0].get(), s.stream);
+                launch_coord_rows_pos(ps.d_gpos[0].get(), n, (int)pr.op - MDGPU_OP_COORD_X, pr.d_temporal.get(), frame0, B, s.stream);
                 break;
             }
-            launch_coord_rows(fr, didx[0], (uint32_t)pr.h_idx[0].size(), (int)pr.op - MDGPU_OP_COORD_X, pr.d_temporal, frame0, s.stream);
+            launch_coord_rows(fr, didx[0], (uint32_t)pr.h_idx[0].size(), (int)pr.op - MDGPU_OP_COORD_X, pr.d_temporal.get(), frame0, s.stream);
             break;
         case MDGPU_OP_SHAPE_WEIGHTS: {
             ShapeArgs a{};
-            a.frames = fr; a.cells = s.d_cells; a.mass = dmass; a.use_mass = (int)(pr.com_mask & 1u);
-            a.idx = didx[0]; a.soff = pr.d_soff; a.n_struct = (uint32_t)pr.n_struct; a.n_atoms_total = (uint32_t)pr.h_idx[0].size();
-            a.scratch_xyzw = ps.d_sdf_xyzw; a.out = pr.d_temporal; a.frame0 = frame0;
+            a.frames = fr; a.cells = s.d_cells.get(); a.mass = dmass; a.use_mass = (int)(pr.com_mask & 1u);
+            a.idx = didx[0]; a.soff = pr.d_soff.get(); a.n_struct = (uint32_t)pr.n_struct; a.n_atoms_total = (uint32_t)pr.h_idx[0].size();
+            a.scratch_xyzw = ps.d_sdf_xyzw.get(); a.out = pr.d_temporal.get(); a.frame0 = frame0;
             launch_shape_weights(a, B, s.stream);
             break; }
         case MDGPU_OP_PLANE: {
             RmsdArgs a{};
-            a.frames = fr; a.cells = s.d_cells; a.mass = dmass; a.idx = didx[0]; a.n = (uint32_t)pr.h_idx[0].size();
+            a.frames = fr; a.cells = s.d_cells.get(); a.mass = dmass; a.idx = didx[0]; a.n = (uint32_t)pr.h_idx[0].size();
             if (!pr.h_goff[0].empty()) {
                 a.n = (uint32_t)pr.h_goff[0].size() - 1;
-                launch_group_com(fr, didx[0], pr.d_goff[0], a.n, dmass, ps.d_gpos[0], s.stream); a.pos = ps.d_gpos[0];
+                launch_group_com(fr, didx[0], pr.d_goff[0].get(), a.n, dmass, ps.d_gpos[0].get(), s.stream); a.pos = ps.d_gpos[0].get();
             }
-            a.unwrap_pairs = pr.d_unwrap; a.n_unwrap = pr.n_unwrap; a.scratch_xyzw = ps.d_sdf_xyzw; a.out = pr.d_temporal; a.frame0 = frame0;
+            a.unwrap_pairs = pr.d_unwrap.get(); a.n_unwrap = pr.n_unwrap; a.scratch_xyzw = ps.d_sdf_xyzw.get(); a.out = pr.d_temporal.get(); a.frame0 = frame0;
             launch_plane(a, B, s.stream);
             break; }
         case MDGPU_OP_DISTANCE_PAIR: {
             uint32_t cnt[2];
             for (int k = 0; k < 2; ++k) {
                 cnt[k] = (uint32_t)(pr.h_goff[k].empty() ? pr.h_idx[k].size() : pr.h_goff[k].size() - 1);
-                if (!pr.h_goff[k].empty()) launch_group_com(fr, didx[k], pr.d_goff[k], cnt[k], dmass, ps.d_gpos[k], s.stream);   // extract_com :857, as for rdf's group references
+                if (!pr.h_goff[k].empty()) launch_group_com(fr, didx[k], pr.d_goff[k].get(), cnt[k], dmass, ps.d_gpos[k].get(), s.stream);   // extract_com :857, as for rdf's group references
             }
-            launch_distance_pair(fr, s.d_cells, didx[0], cnt[0], didx[1], cnt[1], ps.d_gpos[0], ps.d_gpos[1], pr.d_temporal, frame0, s.stream);
+            launch_distance_pair(fr, s.d_cells.get(), didx[0], cnt[0], didx[1], cnt[1], ps.d_gpos[0].get(), ps.d_gpos[1].get(), pr.d_temporal.get(), frame0, s.stream);
             break; }
         case MDGPU_OP_POROSITY:   // sub-batches of PORO_FRAMES frames through the slot's grids
             for (uint32_t f0 = 0; f0 < (uint32_t)B; f0 += PORO_FRAMES) {
                 const uint32_t nf = std::min<uint32_t>(PORO_FRAMES, (uint32_t)B - f0);
                 PorosityArgs a{};
-                a.frames = BatchFrames{ fr.xyz + (size_t)f0 * fr.frame_stride, fr.frame_stride, fr.axis_stride, nf }; a.cells = s.d_cells + f0;
-                a.idx = didx[0]; a.n = (uint32_t)pr.h_idx[0].size(); a.radius = c ? p->d_radius_c : p->d_radius;
-                a.xyzr = ps.d_poro_xyzr; a.hdr = ps.d_poro_hdr; a.grid = ps.d_poro_grid; a.count = ps.d_poro_count;
-                a.frame_set = pr.d_frame_total; a.frame_n = pr.d_frame_n; a.out = pr.d_temporal; a.frame0 = frame0 + f0;
+                a.frames = BatchFrames{ fr.xyz + (size_t)f0 * fr.frame_stride, fr.frame_stride, fr.axis_stride, nf }; a.cells = s.d_cells.get() + f0;
+                a.idx = didx[0]; a.n = (uint32_t)pr.h_idx[0].size(); a.radius = c ? p->d_radius_c.get() : p->d_radius.get();
+                a.xyzr = ps.d_poro_xyzr.get(); a.hdr = ps.d_poro_hdr.get(); a.grid = ps.d_poro_grid.get(); a.count = ps.d_poro_count.get();
+                a.frame_set = pr.d_frame_total.get(); a.frame_n = pr.d_frame_n.get(); a.out = pr.d_temporal.get(); a.frame0 = frame0 + f0;
                 launch_porosity(a, (int)nf, s.stream);
             }
             break;
         case MDGPU_OP_RMSD: {
             if (!p->have_init) return fail(MDGPU_ERR_INVALID_ARG, "rmsd '%s' needs the initial frame (mdgpu_plan_set_initial_frame)", pr.name.c_str());
             RmsdArgs a{};
-            a.frames = fr; a.cells = s.d_cells; a.init_xyz = dinit; a.init_axis_stride = init_as; a.mass = dmass;
-            a.idx = didx[0]; a.n = (uint32_t)pr.h_idx[0].size(); a.unwrap_pairs = pr.d_unwrap; a.n_unwrap = pr.n_unwrap;
-            a.scratch_xyzw = ps.d_sdf_xyzw; a.out = pr.d_temporal; a.frame0 = frame0;
+            a.frames = fr; a.cells = s.d_cells.get(); a.init_xyz = dinit; a.init_axis_stride = init_as; a.mass = dmass;
+            a.idx = didx[0]; a.n = (uint32_t)pr.h_idx[0].size(); a.unwrap_pairs = pr.d_unwrap.get(); a.n_unwrap = pr.n_unwrap;
+            a.scratch_xyzw = ps.d_sdf_xyzw.get(); a.out = pr.d_temporal.get(); a.frame0 = frame0;
             launch_rmsd(a, B, s.stream);
             break; }
         case MDGPU_OP_DISTANCE_MIN: case MDGPU_OP_DISTANCE_MAX:   // both evaluate md_util_min_distance (md_script_functions.inl:3904, 3944)
@@ -1110,22 +1126,22 @@ static int enqueue_batch(mdgpu_plan* p, Slot& s, const BatchFrames& fr, uint32_t
                 uint32_t cnt[2];
                 for (int k = 0; k < 2; ++k) {
                     cnt[k] = (uint32_t)(pr.h_goff[k].empty() ? pr.h_idx[k].size() : pr.h_goff[k].size() - 1);
-                    if (!pr.h_goff[k].empty()) launch_group_com(fr, didx[k], pr.d_goff[k], cnt[k], dmass, ps.d_gpos[k], s.stream);
+                    if (!pr.h_goff[k].empty()) launch_group_com(fr, didx[k], pr.d_goff[k].get(), cnt[k], dmass, ps.d_gpos[k].get(), s.stream);
                 }
-                launch_min_distance_pos(fr, s.d_cells, didx[0], cnt[0], didx[1], cnt[1], ps.d_gpos[0], ps.d_gpos[1], pr.d_temporal, frame0, s.stream);
+                launch_min_distance_pos(fr, s.d_cells.get(), didx[0], cnt[0], didx[1], cnt[1], ps.d_gpos[0].get(), ps.d_gpos[1].get(), pr.d_temporal.get(), frame0, s.stream);
                 break;
             }
-            launch_min_distance(fr, s.d_cells, didx[0], (uint32_t)pr.h_idx[0].size(), didx[1], (uint32_t)pr.h_idx[1].size(), pr.d_temporal, frame0, s.stream, dsel[0], dsel[1]);
+            launch_min_distance(fr, s.d_cells.get(), didx[0], (uint32_t)pr.h_idx[0].size(), didx[1], (uint32_t)pr.h_idx[1].size(), pr.d_temporal.get(), frame0, s.stream, dsel[0], dsel[1]);
             break;
         case MDGPU_OP_DISTANCE: case MDGPU_OP_ANGLE: case MDGPU_OP_DIHEDRAL: {
             TemporalArgs a{};
-            a.frames = fr; a.cells = s.d_cells; a.op = (int)pr.op; a.out = pr.d_temporal; a.frame0 = frame0;
+            a.frames = fr; a.cells = s.d_cells.get(); a.op = (int)pr.op; a.out = pr.d_temporal.get(); a.frame0 = frame0;
             if (pr.n_struct) {
                 for (int k = 0; k < 4; ++k) {
                     a.ctx_idx[k] = didx[k]; a.ctx_pos[k] = nullptr;
                     if (!pr.h_aoff[k].empty()) {   // a selection inside the contexts: one centre of mass per context
-                        launch_arg_com_parts(fr, s.d_cells, didx[k], pr.d_aoff[k], (uint32_t)pr.n_struct, dmass, ps.d_parts[k], s.stream);
-                        a.ctx_pos[k] = ps.d_parts[k];
+                        launch_arg_com_parts(fr, s.d_cells.get(), didx[k], pr.d_aoff[k].get(), (uint32_t)pr.n_struct, dmass, ps.d_parts[k].get(), s.stream);
+                        a.ctx_pos[k] = ps.d_parts[k].get();
                     }
                 }
                 a.n_ctx = (uint32_t)pr.n_struct;
@@ -1133,7 +1149,7 @@ static int enqueue_batch(mdgpu_plan* p, Slot& s, const BatchFrames& fr, uint32_t
                 break;
             }
             for (int k = 0; k < 4; ++k) a.atom[k] = pr.h_idx[k].empty() ? 0 : (c ? pr.first_c[k] : pr.h_idx[k][0]);
-            a.pos = ps.d_argpos; a.com_mask = pr.com_mask;
+            a.pos = ps.d_argpos.get(); a.com_mask = pr.com_mask;
             for (int k = 0; k < 4; ++k) if (pr.com_mask & (1u << k)) arg_position(pr, ps, k, fr, s, didx, dmass, dsel[k]);
             launch_temporal(a, B, s.stream);
             break; }
@@ -1142,7 +1158,7 @@ static int enqueue_batch(mdgpu_plan* p, Slot& s, const BatchFrames& fr, uint32_t
         pr.frames_accumulated += (uint64_t)B;
     }
     CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaMemcpyAsync(s.h_err, s.d_err, sizeof(int), cudaMemcpyDeviceToHost, s.stream));   // read when the slot is retired
+    CUDA_TRY(cudaMemcpyAsync(s.h_err.get(), s.d_err.get(), sizeof(int), cudaMemcpyDeviceToHost, s.stream));   // read when the slot is retired
     CUDA_TRY(cudaEventRecord(s.done, s.stream));
     s.busy = true; s.pending_beg = frame0; s.pending_cnt = (uint32_t)B;
     p->dirty = true;
@@ -1168,9 +1184,9 @@ static int retire_slot(mdgpu_plan* p, Slot& s) {
     if (!s.busy) return 0;
     CUDA_TRY(cudaEventSynchronize(s.done));
     s.busy = false;
-    if (s.h_err && *s.h_err) {
-        const int err = *s.h_err; *s.h_err = 0;
-        cudaMemsetAsync(s.d_err, 0, sizeof(int), s.stream); cudaStreamSynchronize(s.stream);
+    if (s.h_err.get() && *s.h_err.get()) {
+        const int err = *s.h_err.get(); *s.h_err.get() = 0;
+        cudaMemsetAsync(s.d_err.get(), 0, sizeof(int), s.stream); cudaStreamSynchronize(s.stream);
         return device_error(p, err);
     }
     mark_frames(p, s.pending_beg, s.pending_cnt);
@@ -1287,32 +1303,20 @@ static int multi_sync(mdgpu_plan* p) {
     { int rc = nccl_load(m->nccl); if (rc) return rc; }
     if (m->comms.empty()) { m->comms.assign(G, nullptr); NCCL_TRY(m, m->nccl.CommInitAll(m->comms.data(), (int)G, m->devices.data())); }
     cudaEvent_t t0 = nullptr, t1 = nullptr; cudaEventCreate(&t0); cudaEventCreate(&t1); cudaEventRecord(t0, 0);
-    const size_t F = p->num_frames; const size_t NV = (size_t)MDGPU_VOL_DIM * MDGPU_VOL_DIM * MDGPU_VOL_DIM;
     NCCL_TRY(m, m->nccl.GroupStart());
     for (size_t i = 0; i < p->props.size(); ++i) {
-        struct Buf { void* ptr[64]; size_t count; int type; };
-        auto reduce = [&](auto member, size_t count, int type) -> int {
-            if (!(p->props[i].*member)) return 0;
+        // rows of frames a device did not evaluate are zero: the sum merges them (float temporal rows: x + 0 is exact)
+        NCCL_TRY(m, Prop::for_each_accumulator([&](auto member) -> int {
+            const auto& root = p->props[i].*member;
+            if (!root.get()) return 0;
             for (size_t g = 0; g < G; ++g) {
-                mdgpu_plan* q = g ? m->peers[g - 1] : p; void* buf = (void*)(q->props[i].*member);
+                mdgpu_plan* q = g ? m->peers[g - 1] : p; void* buf = (q->props[i].*member).get();
                 cudaSetDevice(q->device);
-                const int r = m->nccl.Reduce(buf, buf, count, type, NCCL_SUM, 0, m->comms[g], 0);
+                const int r = m->nccl.Reduce(buf, buf, root.size(), nccl_type<typename std::remove_reference_t<decltype(root)>::value_type>(), NCCL_SUM, 0, m->comms[g], 0);
                 if (r != 0) return r;
             }
             return 0;
-        };
-        const Prop& pr = p->props[i];
-        NCCL_TRY(m, reduce(&Prop::d_acc, MDGPU_DIST_BINS, NCCL_UINT64));
-        NCCL_TRY(m, reduce(&Prop::d_vol, NV, NCCL_UINT32));
-        NCCL_TRY(m, reduce(&Prop::d_frame_total, F, NCCL_UINT64));
-        NCCL_TRY(m, reduce(&Prop::d_frame_n, F, NCCL_UINT64));
-        NCCL_TRY(m, reduce(&Prop::d_frame_min, F, NCCL_UINT32));   // rows of frames a device did not evaluate are zero: the sum merges them
-        NCCL_TRY(m, reduce(&Prop::d_frame_max, F, NCCL_UINT32));
-        NCCL_TRY(m, reduce(&Prop::d_frame_min64, F, NCCL_UINT64));
-        NCCL_TRY(m, reduce(&Prop::d_frame_max64, F, NCCL_UINT64));
-        NCCL_TRY(m, reduce(&Prop::d_keep, F * MDGPU_DIST_BINS, NCCL_UINT32));
-        NCCL_TRY(m, reduce(&Prop::d_keep64, F * MDGPU_DIST_BINS, NCCL_UINT64));
-        NCCL_TRY(m, reduce(&Prop::d_temporal, F * pr.len, NCCL_FLOAT32));   // disjoint rows, zero elsewhere: x + 0 is exact
+        }));
     }
     NCCL_TRY(m, m->nccl.GroupEnd());
     for (auto* q : m->peers) { CUDA_TRY(cudaSetDevice(q->device)); CUDA_TRY(cudaDeviceSynchronize()); }
@@ -1320,19 +1324,7 @@ static int multi_sync(mdgpu_plan* p) {
     { float ms = 0; if (cudaEventElapsedTime(&ms, t0, t1) == cudaSuccess) { m->last_reduce_ms = ms; m->reduces++; } cudaEventDestroy(t0); cudaEventDestroy(t1); }
     for (auto* q : m->peers) {   // moved, not copied: zero the peers so the next exchange does not count them again
         CUDA_TRY(cudaSetDevice(q->device));
-        for (auto& pr : q->props) {
-            if (pr.d_acc) CUDA_TRY(cudaMemset(pr.d_acc, 0, sizeof(unsigned long long) * MDGPU_DIST_BINS));
-            if (pr.d_vol) CUDA_TRY(cudaMemset(pr.d_vol, 0, sizeof(uint32_t) * NV));
-            if (pr.d_frame_total) CUDA_TRY(cudaMemset(pr.d_frame_total, 0, sizeof(unsigned long long) * F));
-            if (pr.d_frame_n) CUDA_TRY(cudaMemset(pr.d_frame_n, 0, sizeof(unsigned long long) * F));
-            if (pr.d_frame_min) CUDA_TRY(cudaMemset(pr.d_frame_min, 0, sizeof(uint32_t) * F));
-            if (pr.d_frame_max) CUDA_TRY(cudaMemset(pr.d_frame_max, 0, sizeof(uint32_t) * F));
-            if (pr.d_frame_min64) CUDA_TRY(cudaMemset(pr.d_frame_min64, 0, sizeof(unsigned long long) * F));
-            if (pr.d_frame_max64) CUDA_TRY(cudaMemset(pr.d_frame_max64, 0, sizeof(unsigned long long) * F));
-            if (pr.d_keep) CUDA_TRY(cudaMemset(pr.d_keep, 0, sizeof(uint32_t) * F * MDGPU_DIST_BINS));
-            if (pr.d_keep64) CUDA_TRY(cudaMemset(pr.d_keep64, 0, sizeof(unsigned long long) * F * MDGPU_DIST_BINS));
-            if (pr.d_temporal) CUDA_TRY(cudaMemset(pr.d_temporal, 0, sizeof(float) * F * pr.len));
-        }
+        for (auto& pr : q->props) { const int rc = zero_accumulators(pr); if (rc) return rc; }
         p->frames_retired.fetch_add(q->frames_retired.exchange(0));
         std::lock_guard<std::mutex> la(p->mask_mutex); std::lock_guard<std::mutex> lb(q->mask_mutex);
         for (size_t w = 0; w < p->frame_mask.size(); ++w) { p->frame_mask[w] |= q->frame_mask[w]; q->frame_mask[w] = 0; }
@@ -1395,31 +1387,31 @@ static int eval_host_frames_1(mdgpu_plan* p, const float* h_xyz, size_t frame_st
         const float* src = h_xyz + (size_t)b0 * frame_stride;
         cudaError_t e = cudaSuccess;
         if (c) {
-            float* dst = s->h_frames; const int32_t* idx = p->needed.data();
+            float* dst = s->h_frames.get(); const int32_t* idx = p->needed.data();
             ingest_pool(p)->parallel_for(nb * 3, [&](uint32_t w) {
                 const uint32_t i = w / 3, ax = w % 3;
                 gather_axis(dst + ((size_t)i * 3 + ax) * AS, src + (size_t)i * frame_stride + (size_t)ax * axis_stride, idx, M);
             });
-            e = cudaMemcpyAsync(s->d_frames, s->h_frames, sizeof(float) * (size_t)nb * 3 * AS, cudaMemcpyHostToDevice, s->stream);
+            e = cudaMemcpyAsync(s->d_frames.get(), s->h_frames.get(), sizeof(float) * (size_t)nb * 3 * AS, cudaMemcpyHostToDevice, s->stream);
         } else if (pinned) {
             if (frame_stride == 3 * axis_stride && axis_stride == AS && AS == N) {   // fully contiguous: one linear DMA
-                e = cudaMemcpyAsync(s->d_frames, src, sizeof(float) * (size_t)nb * 3 * AS, cudaMemcpyHostToDevice, s->stream);
+                e = cudaMemcpyAsync(s->d_frames.get(), src, sizeof(float) * (size_t)nb * 3 * AS, cudaMemcpyHostToDevice, s->stream);
             } else if (frame_stride == 3 * axis_stride) {
-                e = cudaMemcpy2DAsync(s->d_frames, sizeof(float) * AS, src, sizeof(float) * axis_stride, sizeof(float) * N, (size_t)nb * 3, cudaMemcpyHostToDevice, s->stream);
+                e = cudaMemcpy2DAsync(s->d_frames.get(), sizeof(float) * AS, src, sizeof(float) * axis_stride, sizeof(float) * N, (size_t)nb * 3, cudaMemcpyHostToDevice, s->stream);
             } else {
                 for (uint32_t i = 0; i < nb && e == cudaSuccess; ++i)
-                    e = cudaMemcpy2DAsync(s->d_frames + (size_t)i * 3 * AS, sizeof(float) * AS, src + (size_t)i * frame_stride, sizeof(float) * axis_stride,
+                    e = cudaMemcpy2DAsync(s->d_frames.get() + (size_t)i * 3 * AS, sizeof(float) * AS, src + (size_t)i * frame_stride, sizeof(float) * axis_stride,
                                           sizeof(float) * N, 3, cudaMemcpyHostToDevice, s->stream);
             }
             if (e == cudaSuccess) e = cudaEventRecord(s->copied, s->stream);
             if (std::find(direct.begin(), direct.end(), s->copied) == direct.end()) direct.push_back(s->copied);
         } else {
             for (uint32_t i = 0; i < nb; ++i) for (int ax = 0; ax < 3; ++ax)
-                memcpy(s->h_frames + ((size_t)i * 3 + ax) * AS, src + (size_t)i * frame_stride + (size_t)ax * axis_stride, sizeof(float) * N);
-            e = cudaMemcpyAsync(s->d_frames, s->h_frames, sizeof(float) * (size_t)nb * 3 * AS, cudaMemcpyHostToDevice, s->stream);
+                memcpy(s->h_frames.get() + ((size_t)i * 3 + ax) * AS, src + (size_t)i * frame_stride + (size_t)ax * axis_stride, sizeof(float) * N);
+            e = cudaMemcpyAsync(s->d_frames.get(), s->h_frames.get(), sizeof(float) * (size_t)nb * 3 * AS, cudaMemcpyHostToDevice, s->stream);
         }
         if (e != cudaSuccess) { release_slot(p, s); return fail(MDGPU_ERR_CUDA, "H2D copy failed: %s", cudaGetErrorString(e)); }
-        BatchFrames fr{ s->d_frames, 3 * AS, AS, nb };
+        BatchFrames fr{ s->d_frames.get(), 3 * AS, AS, nb };
         rc = enqueue_batch(p, *s, fr, frame_beg + b0, c);
         release_slot(p, s);
         if (rc) return rc;
@@ -1450,23 +1442,22 @@ static bool xtc_header_cell(const uint8_t* fr, size_t nbytes, mdgpu_unitcell_t* 
     return true;
 }
 
+// the stage is built whole (a stage with a stream is complete) or not at all, so a failed set-up is repeated by the next call
 static int ensure_xtc_stage(mdgpu_plan* p, XtcStage& st, size_t need_bytes) {
     const size_t nf = (size_t)p->B * XTC_SUPER;
     if (!st.stream) {
-        CUDA_TRY(cudaStreamCreateWithFlags(&st.stream, cudaStreamNonBlocking));
-        CUDA_TRY(cudaEventCreateWithFlags(&st.ready, cudaEventDisableTiming));
-        for (auto& e : st.consumed) CUDA_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-        CUDA_TRY(dalloc(&st.d_off, nf + 1));
-        CUDA_TRY(cudaMallocHost((void**)&st.h_off, sizeof(unsigned long long) * (nf + 1)));
-        CUDA_TRY(dalloc(&st.d_info, nf));
-        CUDA_TRY(dalloc(&st.d_rec, nf * p->num_atoms));
-        CUDA_TRY(dalloc(&st.d_state, nf * p->num_atoms));
+        XtcStage b;
+        CUDA_TRY(cudaStreamCreateWithFlags(b.stream.out(), cudaStreamNonBlocking));
+        CUDA_TRY(cudaEventCreateWithFlags(b.ready.out(), cudaEventDisableTiming));
+        for (auto& e : b.consumed) CUDA_TRY(cudaEventCreateWithFlags(e.out(), cudaEventDisableTiming));
+        CUDA_TRY(b.d_off.alloc(nf + 1));
+        CUDA_TRY(b.h_off.alloc(nf + 1));
+        CUDA_TRY(b.d_info.alloc(nf));
+        CUDA_TRY(b.d_rec.alloc(nf * p->num_atoms));
+        CUDA_TRY(b.d_state.alloc(nf * p->num_atoms));
+        st = std::move(b);
     }
-    if (need_bytes + 32 > st.cap) {
-        cudaFree(st.d_blob); st.d_blob = nullptr; st.cap = 0;
-        const size_t cap = std::max(need_bytes + 32, nf * (p->num_atoms * 6 + 128)) + 4096;
-        CUDA_TRY(cudaMalloc((void**)&st.d_blob, cap)); st.cap = cap;
-    }
+    if (need_bytes + 32 > st.d_blob.size()) CUDA_TRY(st.d_blob.alloc(std::max(need_bytes + 32, nf * (p->num_atoms * 6 + 128)) + 4096));
     return 0;
 }
 
@@ -1494,10 +1485,10 @@ int mdgpu_eval_xtc_frames(mdgpu_plan* p, const uint8_t* h_blob, const uint64_t* 
         for (uint32_t q = 0; q < st.n_consumed; ++q) CUDA_TRY(cudaStreamWaitEvent(st.stream, st.consumed[q], 0));   // ... and its bytes expanded
         st.n_consumed = 0;
         for (uint32_t i = 0; i <= ns; ++i) st.h_off[i] = frame_offsets[s0 + i] - beg;
-        CUDA_TRY(cudaMemcpyAsync(st.d_blob, h_blob + beg, (size_t)(end - beg), cudaMemcpyHostToDevice, st.stream));
-        CUDA_TRY(cudaMemsetAsync(st.d_blob + (end - beg), 0, 32, st.stream));   // guard bytes for the word-wise bit reader
-        CUDA_TRY(cudaMemcpyAsync(st.d_off, st.h_off, sizeof(unsigned long long) * (ns + 1), cudaMemcpyHostToDevice, st.stream));
-        launch_xtc_scan(st.d_blob, st.d_off, (uint32_t)NA, (int)ns, st.d_info, st.d_rec, st.d_state, NA, st.stream);
+        CUDA_TRY(cudaMemcpyAsync(st.d_blob.get(), h_blob + beg, (size_t)(end - beg), cudaMemcpyHostToDevice, st.stream));
+        CUDA_TRY(cudaMemsetAsync(st.d_blob.get() + (end - beg), 0, 32, st.stream));   // guard bytes for the word-wise bit reader
+        CUDA_TRY(cudaMemcpyAsync(st.d_off.get(), st.h_off.get(), sizeof(unsigned long long) * (ns + 1), cudaMemcpyHostToDevice, st.stream));
+        launch_xtc_scan(st.d_blob.get(), st.d_off.get(), (uint32_t)NA, (int)ns, st.d_info.get(), st.d_rec.get(), st.d_state.get(), NA, st.stream);
         CUDA_TRY(cudaEventRecord(st.ready, st.stream));
         return 0;
     };
@@ -1518,13 +1509,13 @@ int mdgpu_eval_xtc_frames(mdgpu_plan* p, const uint8_t* h_blob, const uint64_t* 
             }
             if (!ok) { release_slot(p, sp); return fail(MDGPU_ERR_FRAME_SOURCE, "XTC: Magic number did not match"); }
             cudaError_t e = cudaSuccess;
-            if (!s.d_xtc_frames) e = dalloc(&s.d_xtc_frames, (size_t)p->B * 3 * AS);   // whole decoded frames (global atom indices)
+            if (!s.d_xtc_frames.get()) e = s.d_xtc_frames.alloc((size_t)p->B * 3 * AS);   // whole decoded frames (global atom indices)
             if (e == cudaSuccess) e = cudaStreamWaitEvent(s.stream, st.ready, 0);
             if (e != cudaSuccess) { release_slot(p, sp); return fail(MDGPU_ERR_CUDA, "XTC stage set-up failed: %s", cudaGetErrorString(e)); }
-            launch_xtc_expand(st.d_blob, st.d_off + b0, (uint32_t)NA, (int)nb, st.d_info + b0, st.d_rec + (size_t)b0 * NA, st.d_state + (size_t)b0 * NA, NA,
-                              s.d_xtc_frames, 3 * AS, AS, s.d_err, s.stream);
+            launch_xtc_expand(st.d_blob.get(), st.d_off.get() + b0, (uint32_t)NA, (int)nb, st.d_info.get() + b0, st.d_rec.get() + (size_t)b0 * NA, st.d_state.get() + (size_t)b0 * NA, NA,
+                              s.d_xtc_frames.get(), 3 * AS, AS, s.d_err.get(), s.stream);
             cudaEventRecord(st.consumed[st.n_consumed++], s.stream);
-            BatchFrames fr{ s.d_xtc_frames, 3 * AS, AS, nb };
+            BatchFrames fr{ s.d_xtc_frames.get(), 3 * AS, AS, nb };
             rc = enqueue_batch(p, s, fr, frame_beg + s0 + b0, false);
             release_slot(p, sp);
             if (rc) return rc;
@@ -1544,27 +1535,22 @@ int mdgpu_eval_xtc_file(mdgpu_plan* p, const char* path, uint32_t frame_beg, uin
     fseek(fp, 0, SEEK_END); const long fsz = ftell(fp); fseek(fp, 0, SEEK_SET);
     if (fsz <= 0) { fclose(fp); return fail(MDGPU_ERR_FRAME_SOURCE, "XTC: Failed extract filesize"); }
     CUDA_TRY(cudaSetDevice(p->device));
-    uint8_t* buf = nullptr;
-    if (cudaMallocHost((void**)&buf, (size_t)fsz) != cudaSuccess) { fclose(fp); return fail(MDGPU_ERR_CUDA, "pinned allocation of %ld bytes failed", fsz); }
-    const size_t got = fread(buf, 1, (size_t)fsz, fp); fclose(fp);
-    int rc = 0;
+    PinnedBuf<uint8_t> buf;
+    if (buf.alloc((size_t)fsz) != cudaSuccess) { fclose(fp); return fail(MDGPU_ERR_CUDA, "pinned allocation of %ld bytes failed", fsz); }
+    const size_t got = fread(buf.get(), 1, (size_t)fsz, fp); fclose(fp);
     std::vector<uint64_t> offs((size_t)fsz / 56 + 2);
     size_t nf = 0, na = 0;
-    do {
-        if (got != (size_t)fsz) { rc = fail(MDGPU_ERR_FRAME_SOURCE, "XTC: Failed to read frame data from file, expected %ld bytes, got %zu bytes", fsz, got); break; }
-        rc = mdgpu_xtc_frame_offsets(buf, (size_t)fsz, offs.data(), offs.size(), &nf, &na); if (rc) break;
-        if (na != p->num_atoms) { rc = fail(MDGPU_ERR_INVALID_ARG, "XTC: Number of atoms in frame header does not match expected number of atoms"); break; }
-        if (frame_beg > frame_end || frame_end > nf) { rc = fail(MDGPU_ERR_INVALID_ARG, "Script eval: Invalid frame range"); break; }
-        if (!p->have_init && nf) {   // initial configuration = frame 0 of the trajectory (md_script.c:5808)
-            std::vector<float> f0(3 * na); mdgpu_unitcell_t c0{};
-            rc = mdgpu_xtc_decode_frames(p->device, buf, offs.data(), 1, na, f0.data(), &c0, nullptr, nullptr); if (rc) break;
-            rc = mdgpu_plan_set_initial_frame(p, f0.data(), f0.data() + na, f0.data() + 2 * na, &c0); if (rc) break;
-        }
-        rc = mdgpu_eval_xtc_frames(p, buf, offs.data() + frame_beg, frame_beg, frame_end - frame_beg); if (rc) break;
-        rc = mdgpu_plan_sync(p);   // the pinned file image must outlive the copies
-    } while (false);
-    cudaFreeHost(buf);
-    return rc;
+    if (got != (size_t)fsz) return fail(MDGPU_ERR_FRAME_SOURCE, "XTC: Failed to read frame data from file, expected %ld bytes, got %zu bytes", fsz, got);
+    int rc = mdgpu_xtc_frame_offsets(buf.get(), (size_t)fsz, offs.data(), offs.size(), &nf, &na); if (rc) return rc;
+    if (na != p->num_atoms) return fail(MDGPU_ERR_INVALID_ARG, "XTC: Number of atoms in frame header does not match expected number of atoms");
+    if (frame_beg > frame_end || frame_end > nf) return fail(MDGPU_ERR_INVALID_ARG, "Script eval: Invalid frame range");
+    if (!p->have_init && nf) {   // initial configuration = frame 0 of the trajectory (md_script.c:5808)
+        std::vector<float> f0(3 * na); mdgpu_unitcell_t c0{};
+        rc = mdgpu_xtc_decode_frames(p->device, buf.get(), offs.data(), 1, na, f0.data(), &c0, nullptr, nullptr); if (rc) return rc;
+        rc = mdgpu_plan_set_initial_frame(p, f0.data(), f0.data() + na, f0.data() + 2 * na, &c0); if (rc) return rc;
+    }
+    rc = mdgpu_eval_xtc_frames(p, buf.get(), offs.data() + frame_beg, frame_beg, frame_end - frame_beg); if (rc) return rc;
+    return mdgpu_plan_sync(p);   // the pinned file image must outlive the copies
 }
 
 // frame starts of an XTC file image (md_xtc_read_frame_offsets_and_times md_xtc.c:436-570): offsets[0..n], offsets[n] = end of the last frame
@@ -1604,24 +1590,19 @@ int mdgpu_xtc_decode_frames(int device, const uint8_t* h_blob, const uint64_t* f
         if (!xtc_header_cell(h_blob + frame_offsets[i], (size_t)(frame_offsets[i + 1] - frame_offsets[i]), &c, &st, &tm)) return fail(MDGPU_ERR_FRAME_SOURCE, "XTC: Magic number did not match");
         if (h_cells) h_cells[i] = c; if (h_steps) h_steps[i] = st; if (h_times) h_times[i] = tm;
     }
-    uint8_t* d_blob = nullptr; unsigned long long* d_off = nullptr; XtcFrameInfo* d_info = nullptr; uint2* d_rec = nullptr; uint16_t* d_state = nullptr; float* d_out = nullptr; int* d_err = nullptr;
-    auto cleanup = [&]() { cudaFree(d_blob); cudaFree(d_off); cudaFree(d_info); cudaFree(d_rec); cudaFree(d_state); cudaFree(d_out); cudaFree(d_err); };
-    int rc = 0;
-    do {
-        if (cudaMalloc((void**)&d_blob, (size_t)(end - beg) + 32) != cudaSuccess || dalloc(&d_off, (size_t)count + 1) != cudaSuccess || dalloc(&d_info, count) != cudaSuccess ||
-            dalloc(&d_rec, (size_t)count * num_atoms) != cudaSuccess || dalloc(&d_state, (size_t)count * num_atoms) != cudaSuccess ||
-            dalloc(&d_out, (size_t)count * 3 * num_atoms) != cudaSuccess || dalloc(&d_err, 1) != cudaSuccess) { rc = fail(MDGPU_ERR_CUDA, "device allocation failed (xtc decode)"); break; }
-        cudaMemset(d_err, 0, sizeof(int)); cudaMemset(d_blob + (end - beg), 0, 32);
-        cudaMemcpy(d_blob, h_blob + beg, (size_t)(end - beg), cudaMemcpyHostToDevice);
-        cudaMemcpy(d_off, off.data(), sizeof(unsigned long long) * (count + 1), cudaMemcpyHostToDevice);
-        launch_xtc_decode(d_blob, d_off, (uint32_t)num_atoms, (int)count, d_info, d_rec, d_state, num_atoms, d_out, 3 * num_atoms, num_atoms, d_err, 0);
-        int err = 0;
-        if (cudaMemcpy(&err, d_err, sizeof(int), cudaMemcpyDeviceToHost) != cudaSuccess) { rc = fail(MDGPU_ERR_CUDA, "xtc decode failed: %s", cudaGetErrorString(cudaGetLastError())); break; }
-        if (err) { rc = fail(MDGPU_ERR_FRAME_SOURCE, "XTC: Failed to decode frame data"); break; }
-        if (cudaMemcpy(h_xyz, d_out, sizeof(float) * (size_t)count * 3 * num_atoms, cudaMemcpyDeviceToHost) != cudaSuccess) { rc = fail(MDGPU_ERR_CUDA, "xtc decode copy failed"); break; }
-    } while (false);
-    cleanup();
-    return rc;
+    DevBuf<uint8_t> d_blob; DevBuf<unsigned long long> d_off; DevBuf<XtcFrameInfo> d_info; DevBuf<uint2> d_rec; DevBuf<uint16_t> d_state; DevBuf<float> d_out; DevBuf<int> d_err;
+    if (d_blob.alloc((size_t)(end - beg) + 32) != cudaSuccess || d_off.alloc((size_t)count + 1) != cudaSuccess || d_info.alloc(count) != cudaSuccess ||
+        d_rec.alloc((size_t)count * num_atoms) != cudaSuccess || d_state.alloc((size_t)count * num_atoms) != cudaSuccess ||
+        d_out.alloc((size_t)count * 3 * num_atoms) != cudaSuccess || d_err.alloc(1) != cudaSuccess) return fail(MDGPU_ERR_CUDA, "device allocation failed (xtc decode)");
+    cudaMemset(d_err.get(), 0, sizeof(int)); cudaMemset(d_blob.get() + (end - beg), 0, 32);
+    cudaMemcpy(d_blob.get(), h_blob + beg, (size_t)(end - beg), cudaMemcpyHostToDevice);
+    cudaMemcpy(d_off.get(), off.data(), sizeof(unsigned long long) * (count + 1), cudaMemcpyHostToDevice);
+    launch_xtc_decode(d_blob.get(), d_off.get(), (uint32_t)num_atoms, (int)count, d_info.get(), d_rec.get(), d_state.get(), num_atoms, d_out.get(), 3 * num_atoms, num_atoms, d_err.get(), 0);
+    int err = 0;
+    if (cudaMemcpy(&err, d_err.get(), sizeof(int), cudaMemcpyDeviceToHost) != cudaSuccess) return fail(MDGPU_ERR_CUDA, "xtc decode failed: %s", cudaGetErrorString(cudaGetLastError()));
+    if (err) return fail(MDGPU_ERR_FRAME_SOURCE, "XTC: Failed to decode frame data");
+    if (cudaMemcpy(h_xyz, d_out.get(), sizeof(float) * (size_t)count * 3 * num_atoms, cudaMemcpyDeviceToHost) != cudaSuccess) return fail(MDGPU_ERR_CUDA, "xtc decode copy failed");
+    return 0;
 }
 
 // md_script_eval_frame_range's frame loop (md_script.c:6573-6612 -> eval_properties :5730): re-entrant on one plan from many threads with
@@ -1671,7 +1652,7 @@ static int eval_trajectory_1(mdgpu_plan* p, const mdgpu_trajectory_i* traj, uint
         auto work = [&](uint32_t t) {
             for (uint32_t i = t; i < nb; i += T) {
                 mdgpu_frame_header_t fh{};
-                float* dst = s.h_frames + (size_t)i * 3 * AS;
+                float* dst = s.h_frames.get() + (size_t)i * 3 * AS;
                 if (c) {
                     float* tmp = scratch[t].data();
                     if (!readers[t].load_frame(readers[t].inst, (int64_t)(b0 + i), &fh, tmp, tmp + ASF, tmp + 2 * ASF)) { failed = 1; return; }
@@ -1683,9 +1664,9 @@ static int eval_trajectory_1(mdgpu_plan* p, const mdgpu_trajectory_i* traj, uint
         if (T == 1) work(0);
         else { std::vector<std::thread> th; for (uint32_t t = 0; t < T; ++t) th.emplace_back(work, t); for (auto& x : th) x.join(); }
         if (failed) { release_slot(p, sp); rc = fail(MDGPU_ERR_FRAME_SOURCE, "Failed to load frame during evaluation"); break; }
-        cudaError_t e = cudaMemcpyAsync(s.d_frames, s.h_frames, sizeof(float) * (size_t)nb * 3 * AS, cudaMemcpyHostToDevice, s.stream);
+        cudaError_t e = cudaMemcpyAsync(s.d_frames.get(), s.h_frames.get(), sizeof(float) * (size_t)nb * 3 * AS, cudaMemcpyHostToDevice, s.stream);
         if (e != cudaSuccess) { release_slot(p, sp); rc = fail(MDGPU_ERR_CUDA, "H2D copy failed: %s", cudaGetErrorString(e)); break; }
-        BatchFrames fr{ s.d_frames, 3 * AS, AS, nb };
+        BatchFrames fr{ s.d_frames.get(), 3 * AS, AS, nb };
         rc = enqueue_batch(p, s, fr, b0, c);
         release_slot(p, sp);
     }
@@ -1724,10 +1705,10 @@ static int fold_accumulators(mdgpu_plan* p, const std::vector<uint32_t>& done, u
         pr.data.frames_accumulated = n;
         if (pr.op == MDGPU_OP_RDF) {
             std::vector<unsigned long long> acc(MDGPU_DIST_BINS), tot(F); std::vector<uint32_t> mn(F), mx(F);
-            CUDA_TRY(cudaMemcpyAsync(acc.data(), pr.d_acc, sizeof(unsigned long long) * MDGPU_DIST_BINS, cudaMemcpyDeviceToHost, st));
-            CUDA_TRY(cudaMemcpyAsync(tot.data(), pr.d_frame_total, sizeof(unsigned long long) * F, cudaMemcpyDeviceToHost, st));
-            CUDA_TRY(cudaMemcpyAsync(mn.data(), pr.d_frame_min, sizeof(uint32_t) * F, cudaMemcpyDeviceToHost, st));
-            CUDA_TRY(cudaMemcpyAsync(mx.data(), pr.d_frame_max, sizeof(uint32_t) * F, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(acc.data(), pr.d_acc.get(), sizeof(unsigned long long) * MDGPU_DIST_BINS, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(tot.data(), pr.d_frame_total.get(), sizeof(unsigned long long) * F, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(mn.data(), pr.d_frame_min.get(), sizeof(uint32_t) * F, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(mx.data(), pr.d_frame_max.get(), sizeof(uint32_t) * F, cudaMemcpyDeviceToHost, st));
             CUDA_TRY(cudaStreamSynchronize(st));
             // mean of the per-frame integer bins: exact sum, one division (the reference keeps a float cumulative moving
             // average, md_script.c:5912-5921, which drifts by ~1e-5 from this value after 4096 frames: tests/test_oracle_golden.py)
@@ -1746,15 +1727,15 @@ static int fold_accumulators(mdgpu_plan* p, const std::vector<uint32_t>& done, u
             }
             pr.data.min_range[0] = pr.cutoff_min; pr.data.max_range[0] = pr.cutoff_max;   // value_range set by internal_rdf :5415
         } else if (pr.op == MDGPU_OP_SDF) {
-            launch_mean_u32(pr.d_vol, pr.d_vol_mean, pr.values.size(), n, st);   // exact mean, one division per voxel, on the device
-            CUDA_TRY(cudaMemcpyAsync(pr.vptr, pr.d_vol_mean, sizeof(float) * pr.values.size(), cudaMemcpyDeviceToHost, st));
+            launch_mean_u32(pr.d_vol.get(), pr.d_vol_mean.get(), pr.values.size(), n, st);   // exact mean, one division per voxel, on the device
+            CUDA_TRY(cudaMemcpyAsync(pr.vptr, pr.d_vol_mean.get(), sizeof(float) * pr.values.size(), cudaMemcpyDeviceToHost, st));
             CUDA_TRY(cudaStreamSynchronize(st));
             // min_value / max_value are never updated for volumes in the reference (md_script.c:5936-5956)
         } else if (pr.op >= MDGPU_OP_DENSITY_X && pr.op <= MDGPU_OP_DENSITY_Z) {
             std::vector<unsigned long long> acc(MDGPU_DIST_BINS), mn(F), mx(F);
-            CUDA_TRY(cudaMemcpyAsync(acc.data(), pr.d_acc, sizeof(unsigned long long) * MDGPU_DIST_BINS, cudaMemcpyDeviceToHost, st));
-            CUDA_TRY(cudaMemcpyAsync(mn.data(), pr.d_frame_min64, sizeof(unsigned long long) * F, cudaMemcpyDeviceToHost, st));
-            CUDA_TRY(cudaMemcpyAsync(mx.data(), pr.d_frame_max64, sizeof(unsigned long long) * F, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(acc.data(), pr.d_acc.get(), sizeof(unsigned long long) * MDGPU_DIST_BINS, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(mn.data(), pr.d_frame_min64.get(), sizeof(unsigned long long) * F, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(mx.data(), pr.d_frame_max64.get(), sizeof(unsigned long long) * F, cudaMemcpyDeviceToHost, st));
             CUDA_TRY(cudaStreamSynchronize(st));
             const double unit = 1.0 / 16777216.0;
             for (int b = 0; b < MDGPU_DIST_BINS; ++b) pr.vptr[b] = n ? (float)(((double)acc[b] * unit / (double)n) * pr.dens_factor) : 0.0f;
@@ -1783,13 +1764,13 @@ static void done_frames(mdgpu_plan* p, std::vector<uint32_t>& done) {
 static int publish_batch(mdgpu_plan* p, uint32_t beg, uint32_t cnt) {
     {
         std::lock_guard<std::mutex> guard(p->sync_mutex);
-        if (!p->pub_stream) CUDA_TRY(cudaStreamCreateWithFlags(&p->pub_stream, cudaStreamNonBlocking));
+        if (!p->pub_stream) CUDA_TRY(cudaStreamCreateWithFlags(p->pub_stream.out(), cudaStreamNonBlocking));
         const uint32_t end = (uint32_t)std::min<size_t>((size_t)beg + cnt, p->num_frames);
-        for (auto& pr : p->props) if (pr.d_temporal && end > beg) {
-            CUDA_TRY(cudaMemcpyAsync(pr.vptr + (size_t)beg * pr.len, pr.d_temporal + (size_t)beg * pr.len, sizeof(float) * (size_t)(end - beg) * pr.len, cudaMemcpyDeviceToHost, p->pub_stream));
+        for (auto& pr : p->props) if (pr.d_temporal.get() && end > beg) {
+            CUDA_TRY(cudaMemcpyAsync(pr.vptr + (size_t)beg * pr.len, pr.d_temporal.get() + (size_t)beg * pr.len, sizeof(float) * (size_t)(end - beg) * pr.len, cudaMemcpyDeviceToHost, p->pub_stream));
         }
         CUDA_TRY(cudaStreamSynchronize(p->pub_stream));
-        for (auto& pr : p->props) if (pr.d_temporal) { for (uint32_t f = beg; f < end; ++f) fold_temporal_rows(pr, f, false); temporal_ranges(pr); pr.data.frames_accumulated = p->frames_retired.load(); }
+        for (auto& pr : p->props) if (pr.d_temporal.get()) { for (uint32_t f = beg; f < end; ++f) fold_temporal_rows(pr, f, false); temporal_ranges(pr); pr.data.frames_accumulated = p->frames_retired.load(); }
         const auto now = std::chrono::steady_clock::now();
         if (now - p->last_pub >= std::chrono::milliseconds(100)) {
             p->last_pub = now;
@@ -1813,8 +1794,8 @@ int mdgpu_plan_sync(mdgpu_plan* p) {
     CUDA_TRY(cudaDeviceSynchronize());
     p->dirty = false;   // batches enqueued from here on set it again
     for (auto& s : p->slots) {
-        int err = 0; CUDA_TRY(cudaMemcpy(&err, s.d_err, sizeof(int), cudaMemcpyDeviceToHost));
-        if (err) { cudaMemset(s.d_err, 0, sizeof(int)); if (s.h_err) *s.h_err = 0; p->dirty = true; return device_error(p, err); }
+        int err = 0; CUDA_TRY(cudaMemcpy(&err, s.d_err.get(), sizeof(int), cudaMemcpyDeviceToHost));
+        if (err) { cudaMemset(s.d_err.get(), 0, sizeof(int)); if (s.h_err.get()) *s.h_err.get() = 0; p->dirty = true; return device_error(p, err); }
     }
     {
         std::lock_guard<std::mutex> tl(p->submit_mutex);
@@ -1824,8 +1805,8 @@ int mdgpu_plan_sync(mdgpu_plan* p) {
     std::vector<uint32_t> done; done_frames(p, done);
     { int rc = fold_accumulators(p, done, p->frames_retired.load(), 0); if (rc) { p->dirty = true; return rc; } }
     const size_t F = p->num_frames;
-    for (auto& pr : p->props) if (pr.d_temporal) {
-        CUDA_TRY(cudaMemcpy(pr.vptr, pr.d_temporal, sizeof(float) * F * pr.len, cudaMemcpyDeviceToHost));
+    for (auto& pr : p->props) if (pr.d_temporal.get()) {
+        CUDA_TRY(cudaMemcpy(pr.vptr, pr.d_temporal.get(), sizeof(float) * F * pr.len, cudaMemcpyDeviceToHost));
         pr.data.min_value = +FLT_MAX; pr.data.max_value = -FLT_MAX;
         for (uint32_t f : done) fold_temporal_rows(pr, f, false);
         temporal_ranges(pr);
@@ -1860,19 +1841,18 @@ int mdgpu_plan_property_histogram(mdgpu_plan* p, size_t prop, uint32_t num_bins,
     if (!p || prop >= p->props.size() || !out_bins || !num_bins) return fail(MDGPU_ERR_INVALID_ARG, "mdgpu_plan_property_histogram: invalid argument");
     int rc = mdgpu_plan_sync(p); if (rc) return rc;
     Prop& pr = p->props[prop];
-    if (!pr.d_temporal) return fail(MDGPU_ERR_INVALID_ARG, "property '%s' is not a temporal", pr.name.c_str());
+    if (!pr.d_temporal.get()) return fail(MDGPU_ERR_INVALID_ARG, "property '%s' is not a temporal", pr.name.c_str());
     const uint32_t dim = (uint32_t)pr.len, rows = aggregate ? 1u : dim;
     std::vector<uint64_t> mask; { std::lock_guard<std::mutex> lk(p->mask_mutex); mask = p->frame_mask; }
-    unsigned long long* d_mask = nullptr; uint32_t* d_counts = nullptr; uint32_t* d_tot = nullptr;
-    auto done = [&](int r) { cudaFree(d_mask); cudaFree(d_counts); cudaFree(d_tot); return r; };
-    if (dalloc(&d_mask, mask.size()) != cudaSuccess || dalloc(&d_counts, (size_t)rows * num_bins) != cudaSuccess || dalloc(&d_tot, rows) != cudaSuccess) return done(fail(MDGPU_ERR_CUDA, "device allocation failed (histogram)"));
-    cudaMemcpy(d_mask, mask.data(), sizeof(uint64_t) * mask.size(), cudaMemcpyHostToDevice);
-    cudaMemset(d_counts, 0, sizeof(uint32_t) * (size_t)rows * num_bins); cudaMemset(d_tot, 0, sizeof(uint32_t) * rows);
+    DevBuf<unsigned long long> d_mask; DevBuf<uint32_t> d_counts, d_tot;
+    if (d_mask.alloc(mask.size()) != cudaSuccess || d_counts.alloc((size_t)rows * num_bins) != cudaSuccess || d_tot.alloc(rows) != cudaSuccess) return fail(MDGPU_ERR_CUDA, "device allocation failed (histogram)");
+    cudaMemcpy(d_mask.get(), mask.data(), sizeof(uint64_t) * mask.size(), cudaMemcpyHostToDevice);
+    cudaMemset(d_counts.get(), 0, d_counts.bytes()); cudaMemset(d_tot.get(), 0, d_tot.bytes());
     const float range_ext = range_max - range_min, inv_range = range_ext > 0.0f ? 1.0f / range_ext : 0.0f;   // src/main.cpp:188-189
-    launch_temporal_histogram(pr.d_temporal, d_mask, (uint32_t)p->num_frames, dim, range_min, range_max, inv_range, num_bins, aggregate, d_counts, d_tot, 0);
+    launch_temporal_histogram(pr.d_temporal.get(), d_mask.get(), (uint32_t)p->num_frames, dim, range_min, range_max, inv_range, num_bins, aggregate, d_counts.get(), d_tot.get(), 0);
     std::vector<uint32_t> counts((size_t)rows * num_bins), tot(rows);
-    if (cudaMemcpy(counts.data(), d_counts, sizeof(uint32_t) * counts.size(), cudaMemcpyDeviceToHost) != cudaSuccess || cudaMemcpy(tot.data(), d_tot, sizeof(uint32_t) * rows, cudaMemcpyDeviceToHost) != cudaSuccess)
-        return done(fail(MDGPU_ERR_CUDA, "histogram copy failed: %s", cudaGetErrorString(cudaGetLastError())));
+    if (cudaMemcpy(counts.data(), d_counts.get(), sizeof(uint32_t) * counts.size(), cudaMemcpyDeviceToHost) != cudaSuccess || cudaMemcpy(tot.data(), d_tot.get(), sizeof(uint32_t) * rows, cudaMemcpyDeviceToHost) != cudaSuccess)
+        return fail(MDGPU_ERR_CUDA, "histogram copy failed: %s", cudaGetErrorString(cudaGetLastError()));
     float min_bin = FLT_MAX, max_bin = -FLT_MAX;
     const float width = range_ext / (float)num_bins;                                  // :213-222
     for (uint32_t i = 0; i < rows; ++i) {
@@ -1880,7 +1860,7 @@ int mdgpu_plan_property_histogram(mdgpu_plan* p, size_t prop, uint32_t num_bins,
         for (uint32_t j = 0; j < num_bins; ++j) { float v = (float)counts[(size_t)i * num_bins + j]; v *= scl; out_bins[(size_t)i * num_bins + j] = v; min_bin = std::min(min_bin, v); max_bin = std::max(max_bin, v); }
     }
     if (out_min_max) { out_min_max[0] = min_bin; out_min_max[1] = max_bin; }
-    return done(0);
+    return 0;
 }
 
 // Radii of the three box passes per axis that approximate a Gaussian of `sigma` texels: boxes_for_gauss(., 3, sigma) of VIAMD's Ramachandran
@@ -1911,37 +1891,36 @@ int mdgpu_plan_rama_density(mdgpu_plan* p, size_t prop, const uint32_t* segments
     std::vector<uint64_t> mask; { std::lock_guard<std::mutex> lk(p->mask_mutex); mask = p->frame_mask; }
     const size_t texels = 512 * 512 * 4;
     RamaArgs a{};
-    unsigned long long* d_mask = nullptr; uint32_t* d_seg = nullptr; unsigned long long* d_counts = nullptr; unsigned long long* d_samples = nullptr; float* d_buf = nullptr;
-    auto done = [&](int r) { cudaFree(d_mask); cudaFree(d_seg); cudaFree(d_counts); cudaFree(d_samples); cudaFree(d_buf); return r; };
-    if (dalloc(&d_mask, mask.size()) != cudaSuccess || upload(&d_seg, segments ? segments + class_offsets[0] : nullptr, n_entries) != cudaSuccess ||
-        dalloc(&d_counts, texels) != cudaSuccess || dalloc(&d_samples, 4) != cudaSuccess || dalloc(&d_buf, 3 * texels) != cudaSuccess)
-        return done(fail(MDGPU_ERR_CUDA, "device allocation failed (rama density)"));
-    if (cudaMemcpy(d_mask, mask.data(), sizeof(uint64_t) * mask.size(), cudaMemcpyHostToDevice) != cudaSuccess) return done(fail(MDGPU_ERR_CUDA, "frame mask upload failed (rama density)"));
-    a.angles = pr.d_temporal; a.n_seg = (uint32_t)pr.backbone_segments; a.seg = d_seg; a.n_entries = n_entries;
+    DevBuf<unsigned long long> d_mask, d_counts, d_samples; DevBuf<uint32_t> d_seg; DevBuf<float> d_buf;
+    if (d_mask.alloc(mask.size()) != cudaSuccess || d_seg.upload(segments ? segments + class_offsets[0] : nullptr, n_entries) != cudaSuccess ||
+        d_counts.alloc(texels) != cudaSuccess || d_samples.alloc(4) != cudaSuccess || d_buf.alloc(3 * texels) != cudaSuccess)
+        return fail(MDGPU_ERR_CUDA, "device allocation failed (rama density)");
+    if (cudaMemcpy(d_mask.get(), mask.data(), sizeof(uint64_t) * mask.size(), cudaMemcpyHostToDevice) != cudaSuccess) return fail(MDGPU_ERR_CUDA, "frame mask upload failed (rama density)");
+    a.angles = pr.d_temporal.get(); a.n_seg = (uint32_t)pr.backbone_segments; a.seg = d_seg.get(); a.n_entries = n_entries;
     for (int c = 0; c < 3; ++c) a.class_end[c] = class_offsets[c + 1] - class_offsets[0];
-    a.frame_beg = frame_beg; a.frame_count = frame_end - frame_beg; a.mask = d_mask;
+    a.frame_beg = frame_beg; a.frame_count = frame_end - frame_beg; a.mask = d_mask.get();
     a.scale = (float)(1.0 / (2.0 * 3.1415926535897932));   // 1.0f / (2.0f * PI) with the double PI of md_common.h:157
-    a.counts = d_counts; a.samples = d_samples; a.buf[0] = d_buf; a.buf[1] = d_buf + texels; a.buf[2] = d_buf + 2 * texels;
+    a.counts = d_counts.get(); a.samples = d_samples.get(); a.buf[0] = d_buf.get(); a.buf[1] = d_buf.get() + texels; a.buf[2] = d_buf.get() + 2 * texels;
     rama_box_radii(a.box, sigma); a.sm_count = p->sm_count;
     launch_rama_density(a, 0);
     uint64_t samples[4] = { 0, 0, 0, 0 };
-    if (cudaMemcpy(out_tex, a.buf[1], sizeof(float) * texels, cudaMemcpyDeviceToHost) != cudaSuccess || cudaMemcpy(samples, d_samples, sizeof(samples), cudaMemcpyDeviceToHost) != cudaSuccess)
-        return done(fail(MDGPU_ERR_CUDA, "rama density failed: %s", cudaGetErrorString(cudaGetLastError())));
+    if (cudaMemcpy(out_tex, a.buf[1], sizeof(float) * texels, cudaMemcpyDeviceToHost) != cudaSuccess || cudaMemcpy(samples, d_samples.get(), sizeof(samples), cudaMemcpyDeviceToHost) != cudaSuccess)
+        return fail(MDGPU_ERR_CUDA, "rama density failed: %s", cudaGetErrorString(cudaGetLastError()));
     for (int c = 0; c < 4; ++c) out_sum[c] = (float)(double)samples[c];   // den_sum: (float) of the task's double sum
-    return done(0);
+    return 0;
 }
 
 int mdgpu_plan_property_counts(mdgpu_plan* p, size_t prop, uint64_t* out, size_t out_len) {
     if (!p || !out || prop >= p->props.size()) return fail(MDGPU_ERR_INVALID_ARG, "mdgpu_plan_property_counts: invalid argument");
     int rc = mdgpu_plan_sync(p); if (rc) return rc;
     Prop& pr = p->props[prop];
-    if (pr.d_acc) {
+    if (pr.d_acc.get()) {
         if (out_len < MDGPU_DIST_BINS) return fail(MDGPU_ERR_INVALID_ARG, "output too small");
-        CUDA_TRY(cudaMemcpy(out, pr.d_acc, sizeof(uint64_t) * MDGPU_DIST_BINS, cudaMemcpyDeviceToHost));
-    } else if (pr.d_vol) {
+        CUDA_TRY(cudaMemcpy(out, pr.d_acc.get(), sizeof(uint64_t) * MDGPU_DIST_BINS, cudaMemcpyDeviceToHost));
+    } else if (pr.d_vol.get()) {
         const size_t nv = (size_t)MDGPU_VOL_DIM * MDGPU_VOL_DIM * MDGPU_VOL_DIM;
         if (out_len < nv) return fail(MDGPU_ERR_INVALID_ARG, "output too small");
-        std::vector<uint32_t> v(nv); CUDA_TRY(cudaMemcpy(v.data(), pr.d_vol, sizeof(uint32_t) * nv, cudaMemcpyDeviceToHost));
+        std::vector<uint32_t> v(nv); CUDA_TRY(cudaMemcpy(v.data(), pr.d_vol.get(), sizeof(uint32_t) * nv, cudaMemcpyDeviceToHost));
         for (size_t i = 0; i < nv; ++i) out[i] = v[i];
     } else return fail(MDGPU_ERR_UNSUPPORTED, "property '%s' has no integer accumulator", pr.name.c_str());
     return 0;
@@ -1953,10 +1932,10 @@ int mdgpu_plan_property_frame_counts(mdgpu_plan* p, size_t prop, uint32_t frame,
     Prop& pr = p->props[prop];
     if (pr.op != MDGPU_OP_RDF) return fail(MDGPU_ERR_UNSUPPORTED, "per-frame counts are kept for rdf properties only");
     if (out_bins) {
-        if (!pr.d_keep) return fail(MDGPU_ERR_INVALID_ARG, "plan was created without keep_frame_results");
-        CUDA_TRY(cudaMemcpy(out_bins, pr.d_keep + (size_t)frame * MDGPU_DIST_BINS, sizeof(uint32_t) * MDGPU_DIST_BINS, cudaMemcpyDeviceToHost));
+        if (!pr.d_keep.get()) return fail(MDGPU_ERR_INVALID_ARG, "plan was created without keep_frame_results");
+        CUDA_TRY(cudaMemcpy(out_bins, pr.d_keep.get() + (size_t)frame * MDGPU_DIST_BINS, sizeof(uint32_t) * MDGPU_DIST_BINS, cudaMemcpyDeviceToHost));
     }
-    if (out_total) { unsigned long long t = 0; CUDA_TRY(cudaMemcpy(&t, pr.d_frame_total + frame, sizeof(t), cudaMemcpyDeviceToHost)); *out_total = t; }
+    if (out_total) { unsigned long long t = 0; CUDA_TRY(cudaMemcpy(&t, pr.d_frame_total.get() + frame, sizeof(t), cudaMemcpyDeviceToHost)); *out_total = t; }
     return 0;
 }
 
@@ -2042,24 +2021,24 @@ int mdgpu_plan_frame_mask(mdgpu_plan* p, uint64_t* out_words, size_t num_words) 
 int mdgpu_plan_property_accum_ptr(mdgpu_plan* p, size_t prop, void** d_ptr, size_t* bytes, uint32_t* elem_bytes) {
     if (!p || prop >= p->props.size() || !d_ptr || !bytes) return fail(MDGPU_ERR_INVALID_ARG, "invalid argument");
     Prop& pr = p->props[prop];
-    if (pr.d_acc) { *d_ptr = pr.d_acc; *bytes = sizeof(unsigned long long) * MDGPU_DIST_BINS; if (elem_bytes) *elem_bytes = 8; }
-    else if (pr.d_vol) { *d_ptr = pr.d_vol; *bytes = sizeof(uint32_t) * MDGPU_VOL_DIM * MDGPU_VOL_DIM * MDGPU_VOL_DIM; if (elem_bytes) *elem_bytes = 4; }
-    else if (pr.d_temporal) { *d_ptr = pr.d_temporal; *bytes = sizeof(float) * p->num_frames * pr.len; if (elem_bytes) *elem_bytes = 4; }   // float rows, zero where not evaluated
-    else return fail(MDGPU_ERR_UNSUPPORTED, "property '%s' has no accumulator", pr.name.c_str());
-    return 0;
+    auto give = [&](const auto& b) { *d_ptr = b.get(); *bytes = b.bytes(); if (elem_bytes) *elem_bytes = (uint32_t)(b.bytes() / b.size()); return 0; };
+    if (pr.d_acc.get()) return give(pr.d_acc);
+    if (pr.d_vol.get()) return give(pr.d_vol);
+    if (pr.d_temporal.get()) return give(pr.d_temporal);   // float rows, zero where not evaluated
+    return fail(MDGPU_ERR_UNSUPPORTED, "property '%s' has no accumulator", pr.name.c_str());
 }
 
 int mdgpu_plan_property_frame_rows(mdgpu_plan* p, size_t prop, uint32_t which, void** d_ptr, size_t* bytes, uint32_t* elem_bytes) {
     if (!p || prop >= p->props.size() || !d_ptr || !bytes || !elem_bytes) return fail(MDGPU_ERR_INVALID_ARG, "invalid argument");
-    Prop& pr = p->props[prop]; const size_t F = p->num_frames;
+    Prop& pr = p->props[prop];
     *d_ptr = nullptr; *bytes = 0; *elem_bytes = 0;
-    if (which == 0 && pr.d_frame_total) { *d_ptr = pr.d_frame_total; *elem_bytes = 8; }
-    else if (which == 1 && pr.d_frame_n) { *d_ptr = pr.d_frame_n; *elem_bytes = 8; }
-    else if (which == 1 && pr.d_frame_min) { *d_ptr = pr.d_frame_min; *elem_bytes = 4; }
-    else if (which == 1 && pr.d_frame_min64) { *d_ptr = pr.d_frame_min64; *elem_bytes = 8; }
-    else if (which == 2 && pr.d_frame_max) { *d_ptr = pr.d_frame_max; *elem_bytes = 4; }
-    else if (which == 2 && pr.d_frame_max64) { *d_ptr = pr.d_frame_max64; *elem_bytes = 8; }
-    *bytes = (size_t)*elem_bytes * F;
+    auto give = [&](const auto& b) { *d_ptr = b.get(); *bytes = b.bytes(); *elem_bytes = (uint32_t)(b.bytes() / b.size()); };
+    if (which == 0 && pr.d_frame_total.get()) give(pr.d_frame_total);
+    else if (which == 1 && pr.d_frame_n.get()) give(pr.d_frame_n);
+    else if (which == 1 && pr.d_frame_min.get()) give(pr.d_frame_min);
+    else if (which == 1 && pr.d_frame_min64.get()) give(pr.d_frame_min64);
+    else if (which == 2 && pr.d_frame_max.get()) give(pr.d_frame_max);
+    else if (which == 2 && pr.d_frame_max64.get()) give(pr.d_frame_max64);
     return 0;   // a property without that row returns a null pointer
 }
 
@@ -2079,7 +2058,7 @@ int mdgpu_plan_set_frames_accumulated(mdgpu_plan* p, size_t prop, uint64_t frame
 int mdgpu_plan_enable_kernel_timing(mdgpu_plan* p, int enable) {
     if (!p) return MDGPU_ERR_INVALID_ARG;
     std::lock_guard<std::mutex> guard(p->submit_mutex);
-    if (enable && !p->d_counters) { CUDA_TRY(cudaSetDevice(p->device)); CUDA_TRY(dalloc(&p->d_counters, 8)); CUDA_TRY(cudaMemset(p->d_counters, 0, sizeof(unsigned long long) * 8)); }
+    if (enable && !p->d_counters.get()) { CUDA_TRY(cudaSetDevice(p->device)); CUDA_TRY(p->d_counters.alloc(8)); CUDA_TRY(cudaMemset(p->d_counters.get(), 0, p->d_counters.bytes())); }
     p->timing = enable != 0; return 0;
 }
 
@@ -2088,7 +2067,7 @@ int mdgpu_plan_kernel_counter(mdgpu_plan* p, uint32_t which, uint64_t* value) {
     if (!p || !value || which >= 8) return fail(MDGPU_ERR_INVALID_ARG, "mdgpu_plan_kernel_counter: invalid argument");
     int rc = mdgpu_plan_sync(p); if (rc) return rc;
     *value = 0;
-    if (p->d_counters) { unsigned long long v = 0; CUDA_TRY(cudaMemcpy(&v, p->d_counters + which, sizeof(v), cudaMemcpyDeviceToHost)); *value = v; }
+    if (p->d_counters.get()) { unsigned long long v = 0; CUDA_TRY(cudaMemcpy(&v, p->d_counters.get() + which, sizeof(v), cudaMemcpyDeviceToHost)); *value = v; }
     return 0;
 }
 
@@ -2105,7 +2084,7 @@ int mdgpu_plan_timer_begin(mdgpu_plan* p) {
     CUDA_TRY(cudaSetDevice(p->device));
     for (auto& s : p->slots) { int rc = retire_slot(p, s); if (rc) return rc; }
     CUDA_TRY(cudaDeviceSynchronize());
-    if (!p->t_begin) CUDA_TRY(cudaEventCreate(&p->t_begin));
+    if (!p->t_begin) CUDA_TRY(cudaEventCreate(p->t_begin.out()));
     // the device is idle: an event on the legacy default stream is reached immediately and precedes everything enqueued later
     CUDA_TRY(cudaEventRecord(p->t_begin, p->slots.empty() ? (cudaStream_t)0 : p->slots[0].stream));
     return 0;
@@ -2114,7 +2093,7 @@ int mdgpu_plan_timer_begin(mdgpu_plan* p) {
 int mdgpu_plan_timer_end(mdgpu_plan* p, double* elapsed_ms) {
     if (!p || !elapsed_ms || !p->t_begin) return fail(MDGPU_ERR_INVALID_ARG, "mdgpu_plan_timer_end without _begin");
     CUDA_TRY(cudaSetDevice(p->device));
-    while (p->t_end.size() < p->slots.size()) { cudaEvent_t e; CUDA_TRY(cudaEventCreate(&e)); p->t_end.push_back(e); }
+    while (p->t_end.size() < p->slots.size()) { Event e; CUDA_TRY(cudaEventCreate(e.out())); p->t_end.push_back(std::move(e)); }
     for (size_t i = 0; i < p->slots.size(); ++i) CUDA_TRY(cudaEventRecord(p->t_end[i], p->slots[i].stream));
     double best = 0.0;
     for (size_t i = 0; i < p->slots.size(); ++i) {
