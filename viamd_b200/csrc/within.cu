@@ -18,15 +18,6 @@ namespace mdg {
 
 constexpr int WITHIN_WARPS = 4;
 
-template <bool TRI>
-MDG_D float within_d2(float dx, float dy, float dz, const FrameGeom& g) {
-    const float dx2 = __fmul_rn(dx, dx), dy2 = __fmul_rn(dy, dy), dz2 = __fmul_rn(dz, dz);
-    const float acc = __fmaf_rn(g.G00, dx2, __fmaf_rn(g.G11, dy2, __fmul_rn(g.G22, dz2)));            // distance_squared_ort_256 :524-529
-    if (!TRI) return acc;
-    const float dxy = __fmul_rn(dx, dy), dxz = __fmul_rn(dx, dz), dyz = __fmul_rn(dy, dz);
-    return __fadd_rn(acc, __fmaf_rn(g.H01, dxy, __fmaf_rn(g.H02, dxz, __fmul_rn(g.H12, dyz))));       // distance_squared_tri_256 :503-515
-}
-
 // One warp per home cell (grid-stride): for every neighbour cell the lanes take its target points 32 at a time and test them against
 // the home cell's reference points until one is within the radius.
 template <bool TRI>
@@ -40,30 +31,18 @@ __global__ void __launch_bounds__(WITHIN_WARPS * 32) k_within_mark(WithinArgs a)
     const float4* __restrict__ ref = a.ref.sorted + (size_t)f * a.ref.max_points;
     const uint32_t* __restrict__ ref_off = a.ref.cell_cnt + (size_t)f * (a.ref.cap + 1);
     uint8_t* __restrict__ flags = a.flags + (size_t)f * a.num_atoms;
-    const int cd0 = g.cdim[0], cd1 = g.cdim[1], cd2 = g.cdim[2], n0 = g.ncell[0], n1 = g.ncell[1], n2 = g.ncell[2];
-    const int w0 = 2 * n0 + 1, w1 = 2 * n1 + 1, w2 = 2 * n2 + 1, nn = w0 * w1 * w2;
-    const uint32_t hd0 = (uint32_t)g.hdim[0], hd1 = (uint32_t)g.hdim[1];
+    const CellWalk w = cell_walk(g);
+    const int nn = walk_size(w);
     const float r2 = g.r2, min_r2 = a.min_r2;
     for (uint32_t h = blockIdx.x * WITHIN_WARPS + warp; h < g.num_home; h += gridDim.x * WITHIN_WARPS) {
         const uint32_t rb = ref_off[h], re = ref_off[h + 1];
         if (rb == re) continue;
-        const int cvx = (int)(h % hd0) + g.hlo[0], cvy = (int)((h / hd0) % hd1) + g.hlo[1], cvz = (int)(h / (hd0 * hd1)) + g.hlo[2];   // unclamped cell of the reference points
+        const int3 c = home_cell(g, h);
         for (int n = 0; n < nn; ++n) {
-            const int ox = n % w0 - n0, oy = (n / w0) % w1 - n1, oz = n / (w0 * w1) - n2;
-            int nx = cvx + ox, ny = cvy + oy, nz = cvz + oz;
-            const bool upx = nx > cd0 - 1, lox = nx < 0, upy = ny > cd1 - 1, loy = ny < 0, upz = nz > cd2 - 1, loz = nz < 0;
-            if (!TRI) {   // wraps on non-periodic axes are skipped (:1733); triclinic cells are periodic in all axes (:1556-1557)
-                if ((upx || lox) && !(g.flags & MDGPU_CELL_PBC_X)) continue;
-                if ((upy || loy) && !(g.flags & MDGPU_CELL_PBC_Y)) continue;
-                if ((upz || loz) && !(g.flags & MDGPU_CELL_PBC_Z)) continue;
-            }
-            nx += lox ? cd0 : 0; nx -= upx ? cd0 : 0;
-            ny += loy ? cd1 : 0; ny -= upy ? cd1 : 0;
-            nz += loz ? cd2 : 0; nz -= upz ? cd2 : 0;
-            if (nx < 0 || nx >= cd0 || ny < 0 || ny >= cd1 || nz < 0 || nz >= cd2) continue;   // the reference wraps once only
-            const uint32_t cj = ((uint32_t)nz * (uint32_t)cd1 + (uint32_t)ny) * (uint32_t)cd0 + (uint32_t)nx;
-            const uint32_t start = trg_off[cj], len = trg_off[cj + 1] - start;
-            const float shx = (float)((lox ? 1 : 0) - (upx ? 1 : 0)), shy = (float)((loy ? 1 : 0) - (upy ? 1 : 0)), shz = (float)((loz ? 1 : 0) - (upz ? 1 : 0));
+            const Neighbour nb = neighbour_cell<TRI>(w, c, n);
+            if (!nb.ok) continue;
+            const uint32_t start = trg_off[nb.cj], len = trg_off[nb.cj + 1] - start;
+            const float3 sh = image_shift(nb.code);
             for (uint32_t j = lane; j < len; j += 32) {
                 const float4 t = trg[start + j];
                 const uint32_t tj = __float_as_uint(t.w);
@@ -71,8 +50,8 @@ __global__ void __launch_bounds__(WITHIN_WARPS * 32) k_within_mark(WithinArgs a)
                 bool hit = false;
                 for (uint32_t i = rb; i < re && !hit; ++i) {
                     const float4 rf = ref[i];
-                    const float fx = __fadd_rn(rf.x, shx), fy = __fadd_rn(rf.y, shy), fz = __fadd_rn(rf.z, shz);   // f + image shift (:1755)
-                    const float d2 = within_d2<TRI>(__fsub_rn(fx, t.x), __fsub_rn(fy, t.y), __fsub_rn(fz, t.z), g);
+                    const float fx = __fadd_rn(rf.x, sh.x), fy = __fadd_rn(rf.y, sh.y), fz = __fadd_rn(rf.z, sh.z);   // f + image shift (:1755)
+                    const float d2 = pair_d2<TRI>(__fsub_rn(fx, t.x), __fsub_rn(fy, t.y), __fsub_rn(fz, t.z), g);
                     hit = d2 <= r2 && d2 >= min_r2;   // within_frng_cb (:2599-2607); min_r2 = 0 for the plain form
                 }
                 if (hit) flags[tj] = 1;
