@@ -11,6 +11,7 @@
 #include "common.cuh"
 #include "kernels.h"
 #include "cellmath.cuh"
+#include "pbcmath.cuh"
 
 namespace mdg {
 
@@ -29,17 +30,7 @@ MDG_HD void compute_frame_geom(FrameGeom& g, const mdgpu_unitcell_t& uc, double 
     A[2][0] = uc.xz; A[2][1] = uc.yz; A[2][2] = uc.z;
     if (!flags) {
         for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) I[i][j] = 0.0;
-    } else {
-        const double i11 = uc.x > 0.0 ? 1.0 / uc.x : 0.0;
-        const double i22 = uc.y > 0.0 ? 1.0 / uc.y : 0.0;
-        const double i33 = uc.z > 0.0 ? 1.0 / uc.z : 0.0;
-        const double i12 = (uc.x * uc.y) > 0.0 ? -uc.xy / (uc.x * uc.y) : 0.0;
-        const double i13 = (uc.x * uc.y * uc.z) > 0.0 ? (uc.xy * uc.yz - uc.xz * uc.y) / (uc.x * uc.y * uc.z) : 0.0;
-        const double i23 = (uc.y * uc.z) > 0.0 ? -uc.yz / (uc.y * uc.z) : 0.0;
-        I[0][0] = i11; I[0][1] = 0.0; I[0][2] = 0.0;
-        I[1][0] = i12; I[1][1] = i22; I[1][2] = 0.0;
-        I[2][0] = i13; I[2][1] = i23; I[2][2] = i33;
-    }
+    } else cell_inverse(uc, I);
     float origin[3] = { 0.f, 0.f, 0.f };
     if ((flags & MDGPU_CELL_PBC_ALL) != MDGPU_CELL_PBC_ALL && aabb) {
         for (int k = 0; k < 3; ++k) {
