@@ -22,6 +22,7 @@
 #include <utility>
 #include <vector>
 #include <map>
+#include <memory>
 #include <algorithm>
 #include <sched.h>
 #include <dlfcn.h>
@@ -104,17 +105,16 @@ struct CellListBuf {
 
 struct Prop {
     std::string name; uint32_t op = 0;
-    std::vector<int32_t> h_idx[4]; DevBuf<int32_t> d_idx[4];
-    DevBuf<int32_t> d_idx_c[4];                    // the same lists in the plan's compact atom space (host ingest of selected atoms)
-    int32_t first_c[4] = { 0, 0, 0, 0 };           // compact index of each list's first atom (single-atom arguments are passed by value)
+    std::vector<int32_t> h_idx[4];
+    DevBuf<int32_t> d_idx[2][4];                   // the lists in each atom space: [SPACE_FULL] global indices, [SPACE_COMPACT] remapped (host ingest of selected atoms)
+    int32_t first[2][4] = {};                      // index of each list's first atom in each space (single-atom arguments are passed by value)
     size_t n_struct = 0, struct_size = 0;
     uint32_t com_mask = 0;   // distance/angle/dihedral: bit k = argument k is a selection evaluated through md_util_com_compute
     std::vector<uint32_t> h_soff; DevBuf<uint32_t> d_soff;   // rdf with centre-of-mass references: CSR offsets of the groups in idx[0]
     float cutoff_min = 0.f, cutoff_max = 0.f;
-    std::vector<uint32_t> h_goff[2]; DevBuf<uint32_t> d_goff[2];   // distance_pair: CSR groups of argument 0 / 1 (arrays of selections)
+    std::vector<uint32_t> h_goff[2]; DevBuf<uint32_t> d_goff[2];   // argument 0 / 1 is an ARRAY of selections, one position per selection: their CSR offsets in idx[k]
     std::vector<uint32_t> h_aoff[4]; DevBuf<uint32_t> d_aoff[4];   // distance / angle / dihedral / com: argument k is an ARRAY of selections (centre of their centres)
     DevBuf<uint8_t> d_and_mask;   // `selection and within(...)`: one byte per atom of the static side (count(within()) / rdf(within()))
-    float ref_within = 0.f, ref_within_min = 0.f;   // (kept for messages) rdf reference given through the round-1 fields; folded into dyn[0]
     // Dynamic arguments: argument k is within([rmin:]rmax, h_idx[k]) [and a static selection], evaluated per frame on the device into an ascending
     // index list (md_script_functions.inl:2485-2720); the consumers read that list instead of the static one.
     struct DynArg { bool on = false; float rmin = 0.f, rmax = 0.f; DevBuf<uint8_t> d_and_mask; } dyn[4];
@@ -137,12 +137,13 @@ struct Prop {
     // results: `values` is the default storage; mdgpu_plan_bind_property_storage points vptr (and the aggregate rows) at the caller's arrays
     // (the md_script shim binds md_script_property_data_t::values, so results are written where VIAMD reads them)
     std::vector<float> values; mdgpu_property_data_t data{};
-    float* vptr = nullptr; float* amean = nullptr; float* avar = nullptr; float* aext = nullptr; bool bound = false;
+    float* vptr = nullptr; float* amean = nullptr; float* avar = nullptr; float* aext = nullptr;
     uint64_t frames_accumulated = 0;    // may be overridden after a cross-GPU reduction
     bool frames_overridden = false;
-    bool is_dist() const { return op == MDGPU_OP_RDF || (op >= MDGPU_OP_DENSITY_X && op <= MDGPU_OP_DENSITY_Z); }
+    bool is_density() const { return op >= MDGPU_OP_DENSITY_X && op <= MDGPU_OP_DENSITY_Z; }
+    bool is_dist() const { return op == MDGPU_OP_RDF || is_density(); }
     bool needs_cells() const { return op == MDGPU_OP_RDF || op == MDGPU_OP_SDF || op == MDGPU_OP_CONTACT_COUNT; }
-    DevBuf<uint32_t> d_set_of;   // contact_count: set of every atom of the concatenated A list
+    DevBuf<uint32_t> d_set_of, d_excl_off;   // contact_count: set of every atom of the concatenated A list; CSR offsets of the sets' exclusion lists in idx[2]
     int share_trg = -1;   // index of an earlier property with the same target selection and cutoff: its target cell list is reused
     size_t trg_groups = 0;   // rdf: the target argument was an ARRAY of selections: one centre of mass per selection is the target point (h_goff[1] = their CSR offsets in idx[1])
     size_t backbone_segments = 0;   // MDGPU_OP_BACKBONE_ANGLES (evaluated as 2 dihedrals in context per segment): the segments of its (phi, psi) rows
@@ -160,6 +161,10 @@ struct Prop {
     }
 };
 
+// One within([rmin:]rmax, selection) query per frame of a batch: the system-wide grid and the cell lists of all atoms and of the selection
+// (get_spatial_acc :734), the marks [B][num_atoms] and, for a dynamic argument, the per-frame index list (empty for count(within())).
+struct WithinScratch { DevBuf<FrameGeom> d_geom; DevBuf<float> d_aabb; CellListBuf trg, ref; DevBuf<uint8_t> d_flags; DevBuf<int32_t> d_idx; DevBuf<uint32_t> d_n; };
+
 struct PropScratch {   // per (stream slot, property)
     DevBuf<FrameGeom> d_geom; DevBuf<float> d_aabb;
     CellListBuf trg, ref;
@@ -167,11 +172,9 @@ struct PropScratch {   // per (stream slot, property)
     DevBuf<float4> d_sdf_xyzw; DevBuf<float> d_sdf_ref0, d_sdf_mats;
     DevBuf<float> d_com;       // rdf with centre-of-mass references: [B][n_struct][3]
     DevBuf<float> d_argpos;    // distance/angle/dihedral with selection arguments: [B][4][3]
-    DevBuf<float> d_gpos[2];   // distance_pair with arrays of selections: [B][n_groups][3] per argument
+    DevBuf<float> d_gpos[2];   // arguments that are arrays of selections: [B][n_groups][3] per argument
     DevBuf<float4> d_parts[4];   // array-of-selections arguments: [B][n_parts] centres (xyz, 1)
-    DevBuf<uint8_t> d_flags;   // count(within()) / rdf(within(), ...): [B][num_atoms]
-    // per dynamic argument: the system-wide grid + lists of its within() query (get_spatial_acc :734), the marks and the per-frame index list
-    struct DynScratch { DevBuf<FrameGeom> d_geom; DevBuf<float> d_aabb; CellListBuf trg, ref; DevBuf<uint8_t> d_flags; DevBuf<int32_t> d_idx; DevBuf<uint32_t> d_n; } dynw[4];
+    WithinScratch within[4];   // the query of dynamic argument k; count(within()) is the query of its argument 0
     // rdf candidate lists (k_rdf_cull): [B][list stride] entries, [B][cap] headers, [B] cursors
     DevBuf<uint32_t> d_pair_list; DevBuf<uint4> d_list_hdr; DevBuf<uint32_t> d_list_cursor;
     mdgpu_unitcell_t nn_cell{}; size_t nn_stride = 0; bool nn_valid = false;   // candidate-list stride of the last cell seen (list sizing)
@@ -240,31 +243,35 @@ struct MultiDevice {
 using namespace mdg;
 
 struct IngestPool;
+// The atoms of a frame as the kernels see them. SPACE_FULL: every atom of the system, global indices. SPACE_COMPACT: the union of the atoms any property reads,
+// ascending: when it is well below the system size, host ingest copies only those atoms (gathered into pinned staging by the ingest threads) and the kernels run on index lists remapped into that space.
+enum Space { SPACE_FULL = 0, SPACE_COMPACT = 1 };
+struct AtomSpace {
+    size_t num_atoms = 0, axis_stride = 0;   // staging layout: [frame][3][axis_stride]
+    DevBuf<float> d_mass, d_init, d_radius;  // masses, the initial frame, van der Waals radii (porosity plans only)
+};
 struct mdgpu_plan {
     int device = 0; int sm_count = 132;
-    size_t num_atoms = 0, num_frames = 0; size_t axis_stride = 0;   // staging layout: [frame][3][axis_stride]
+    size_t num_atoms = 0, num_frames = 0;    // of the system (= space[SPACE_FULL].num_atoms)
     uint32_t B = 132; uint32_t S = 2; uint32_t cell_cap = 0; bool keep = false; uint32_t rdf_variant = 0;
-    std::vector<float> h_mass; DevBuf<float> d_mass;
-    std::vector<float> h_radius; DevBuf<float> d_radius, d_radius_c;   // van der Waals radii (porosity plans only)
-    // Compact atom space: the union of the atoms any property reads, ascending. When it is well below the system size, host ingest copies
-    // only those atoms (gathered into pinned staging by the ingest threads) and the kernels run on index lists remapped into that space.
-    bool compact = false; std::vector<int32_t> needed; size_t num_atoms_c = 0, axis_stride_c = 0; DevBuf<float> d_mass_c, d_init_c;
+    std::vector<float> h_mass, h_radius; AtomSpace space[2];   // space[SPACE_FULL] is always filled, space[SPACE_COMPACT] only when `compact`
+    bool compact = false; std::vector<int32_t> needed;   // host ingest copies only the `needed` atoms
+    Space ingest_space() const { return compact ? SPACE_COMPACT : SPACE_FULL; }
     uint32_t ingest_mode = 0, ingest_threads = 0; IngestPool* pool = nullptr;
     std::vector<uint32_t> conn_off; std::vector<int32_t> conn_idx;
     std::vector<Prop> props;
     std::vector<Slot> slots;
-    bool have_init = false; DevBuf<float> d_init; mdgpu_unitcell_t init_cell{};
+    bool have_init = false; mdgpu_unitcell_t init_cell{};
     std::vector<uint64_t> frame_mask; std::mutex mask_mutex; std::mutex init_mutex;
     std::atomic<bool> interrupt{false};
     uint64_t next_slot = 0;
     // Concurrency (md_script_eval_frame_range is re-entrant on one eval from many threads with disjoint ranges, task_system.cpp:73-87):
-    // a caller thread owns a slot from acquire_slot to release_slot (staging buffers + stream); enqueue_batch runs under submit_mutex;
+    // a caller thread owns a slot (staging buffers + stream) while it holds the lease acquire_slot gave it; enqueue_batch runs under submit_mutex;
     // one fold at a time (sync_mutex).
     std::mutex slot_mutex; std::condition_variable slot_cv; std::mutex submit_mutex; std::mutex sync_mutex;
     mdgpu_progress_fn progress_fn = nullptr; void* progress_user = nullptr; Stream pub_stream;
     std::chrono::steady_clock::time_point last_pub{};
     bool timing = false; std::vector<TimedLaunch> timed; double timed_ms[TIMED_KINDS] = {0, 0, 0, 0}; uint64_t timed_n[TIMED_KINDS] = {0, 0, 0, 0}; DevBuf<unsigned long long> d_counters;
-    bool tri_seen = false, ortho_seen = false;
     Event t_begin; std::vector<Event> t_end;
     XtcStage xtc[XTC_STAGES]; uint64_t next_xtc = 0; std::mutex xtc_mutex;
     std::atomic<bool> dirty{true};   // device accumulators changed since the last fold into the host-visible property data
@@ -436,7 +443,8 @@ mdgpu_plan* mdgpu_plan_create(const mdgpu_system_desc_t* sys, const mdgpu_proper
     p->device = o.device;
     cudaDeviceGetAttribute(&p->sm_count, cudaDevAttrMultiProcessorCount, o.device);
     p->num_atoms = sys->num_atoms; p->num_frames = num_frames;
-    p->axis_stride = (sys->num_atoms + 3) & ~(size_t)3;
+    AtomSpace& full = p->space[SPACE_FULL];
+    full.num_atoms = sys->num_atoms; full.axis_stride = (sys->num_atoms + 3) & ~(size_t)3;
     p->B = o.batch_frames ? o.batch_frames : (uint32_t)p->sm_count;
     if (p->B > 4096) p->B = 4096;
     // 6 slots: the gather + H2D of the batches ahead overlap the kernels of the ones in flight; 2 leave the copy engine idle
@@ -451,20 +459,32 @@ mdgpu_plan* mdgpu_plan_create(const mdgpu_system_desc_t* sys, const mdgpu_proper
         if (sys->bond_conn_atom_idx) p->conn_idx.assign(sys->bond_conn_atom_idx, sys->bond_conn_atom_idx + nconn);
     }
     auto bail = [&](int code, const std::string& msg) -> mdgpu_plan* { fail(code, "%s", msg.c_str()); destroy_plan(p); return nullptr; };
-    // arguments 0 / 1 of distance_pair / distance_min / _max and argument 0 of coord_* given as ARRAYS of selections: one position (centre of mass) per
-    // selection; CSR offsets in structure_offsets (argument 0, num_structures groups) / structure_offsets_b (argument 1)
+    // argument k given as an ARRAY of n selections, one position (centre of mass) per selection: their CSR offsets in idx[k] -> h_goff[k] / d_goff[k].
+    // `who`, `role`, `noun` and `list` word the messages for the site; 0 and "", or the error code and its message
+    auto take_group = [&](Prop& pr, int k, const uint32_t* off, size_t n, const std::string& who, const char* role, const char* noun, const char* list, std::string& er) -> int {
+        if (pr.dyn[k].on) { er = who + ": an array of selections cannot be a dynamic " + role; return MDGPU_ERR_INVALID_ARG; }
+        er = check_offsets(off, n, pr.h_idx[k].size(), who, noun, list); if (!er.empty()) return MDGPU_ERR_INVALID_ARG;
+        pr.h_goff[k].assign(off, off + n + 1);
+        if (pr.d_goff[k].upload(pr.h_goff[k].data(), pr.h_goff[k].size()) != cudaSuccess) { er = std::string("device allocation failed (") + noun + ")"; return MDGPU_ERR_CUDA; }
+        return 0;
+    };
+    // arguments 0 / 1 of distance_pair / distance_min / _max and argument 0 of coord_* / plane given as arrays of selections: CSR offsets in structure_offsets
+    // (argument 0, num_structures groups) / structure_offsets_b (argument 1); cnt[k] = positions of argument k. "" or the message (their callers report every failure as an invalid argument)
     auto take_groups = [&](Prop& pr, const mdgpu_property_desc_t& d, size_t cnt[2]) -> std::string {
         const uint32_t* goff[2] = { d.structure_offsets, d.structure_offsets_b }; const size_t gn[2] = { d.num_structures, d.num_structures_b };
         for (int k = 0; k < 2; ++k) {
-            cnt[k] = pr.h_idx[k].size();
-            if (!gn[k]) continue;
-            if (pr.dyn[k].on) return "'" + pr.name + "': an array of selections cannot be a dynamic argument";
-            const std::string er = check_offsets(goff[k], gn[k], pr.h_idx[k].size(), "'" + pr.name + "'", "group offsets", "the index list"); if (!er.empty()) return er;
-            pr.h_goff[k].assign(goff[k], goff[k] + gn[k] + 1); cnt[k] = gn[k];
-            if (pr.d_goff[k].upload(pr.h_goff[k].data(), pr.h_goff[k].size()) != cudaSuccess) return "device allocation failed (group offsets)";
+            cnt[k] = gn[k] ? gn[k] : pr.h_idx[k].size();
+            std::string er; if (gn[k] && take_group(pr, k, goff[k], gn[k], "'" + pr.name + "'", "argument", "group offsets", "the index list", er)) return er;
         }
         pr.n_struct = 0;   // num_structures described argument 0's groups here, not structures
         return std::string();
+    };
+    // `selection and within(...)`: one byte per atom, 1 for the n atoms of the static side -> d_mask; false after bail()
+    auto take_and_mask = [&](Prop& pr, DevBuf<uint8_t>& d_mask, const int32_t* idx, size_t n) -> bool {
+        std::vector<uint8_t> m(sys->num_atoms, 0);
+        for (size_t j = 0; j < n; ++j) { const int32_t a = idx[j]; if (a < 0 || (size_t)a >= sys->num_atoms) { bail(MDGPU_ERR_INVALID_ARG, "property '" + pr.name + "': atom index out of range"); return false; } m[(size_t)a] = 1; }
+        if (d_mask.upload(m.data(), m.size()) != cudaSuccess) { bail(MDGPU_ERR_CUDA, "device allocation failed (selection mask)"); return false; }
+        return true;
     };
     // argument k of distance / angle / dihedral / com given as an ARRAY of selections (arg_parts[k] >= 2): idx[k] holds them back to back
     auto take_arg_parts = [&](Prop& pr, const mdgpu_property_desc_t& d, int k) -> std::string {
@@ -476,12 +496,12 @@ mdgpu_plan* mdgpu_plan_create(const mdgpu_system_desc_t* sys, const mdgpu_proper
         pr.com_mask |= 1u << k;
         return std::string();
     };
-    if (p->d_mass.upload(p->h_mass.data(), p->h_mass.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (masses)");
+    if (full.d_mass.upload(p->h_mass.data(), p->h_mass.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (masses)");
     for (size_t i = 0; i < num_props; ++i) if (props[i].op == MDGPU_OP_POROSITY) {   // porosity voxelises van der Waals spheres: the radii are required
         if (!sys->atom_radius) return bail(MDGPU_ERR_INVALID_ARG, "porosity: the system description has no atom radii (mdgpu_system_desc_t.atom_radius)");
         p->h_radius.assign(sys->atom_radius, sys->atom_radius + sys->num_atoms);
         for (size_t a = 0; a < sys->num_atoms; ++a) if (!(p->h_radius[a] >= 0.0f && p->h_radius[a] <= FLT_MAX)) return bail(MDGPU_ERR_INVALID_ARG, "porosity: atom radius " + std::to_string(a) + " is negative or not finite");
-        if (p->d_radius.upload(p->h_radius.data(), p->h_radius.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (radii)");
+        if (full.d_radius.upload(p->h_radius.data(), p->h_radius.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (radii)");
         break;
     }
 
@@ -494,7 +514,7 @@ mdgpu_plan* mdgpu_plan_create(const mdgpu_system_desc_t* sys, const mdgpu_proper
             if (d.idx[k] && d.idx_count[k]) {
                 pr.h_idx[k].assign(d.idx[k], d.idx[k] + d.idx_count[k]);
                 for (int32_t a : pr.h_idx[k]) if ((a < 0 && !(pr.op == MDGPU_OP_BACKBONE_ANGLES && a == -1)) || (a >= 0 && (size_t)a >= sys->num_atoms)) return bail(MDGPU_ERR_INVALID_ARG, "property '" + pr.name + "': atom index out of range");
-                if (pr.d_idx[k].upload(pr.h_idx[k].data(), pr.h_idx[k].size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (indices)");
+                if (pr.d_idx[SPACE_FULL][k].upload(pr.h_idx[k].data(), pr.h_idx[k].size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (indices)");
             }
         }
         {   // dynamic arguments (dyn[k]); rdf's round-1 spelling ref_within_radius + com_args bit 0 + idx[2] becomes dyn[0]
@@ -504,41 +524,31 @@ mdgpu_plan* mdgpu_plan_create(const mdgpu_system_desc_t* sys, const mdgpu_proper
                 da[0].and_idx = d.idx[2]; da[0].and_count = d.idx_count[2];
             }
             for (int k = 0; k < 4; ++k) if (da[k].radius_max > 0.0f && pr.op != MDGPU_OP_WITHIN_COUNT) {
-                const bool ok_op = (pr.op == MDGPU_OP_RDF && k < 2) || (pr.op == MDGPU_OP_SDF && k == 1) || (pr.op >= MDGPU_OP_DENSITY_X && pr.op <= MDGPU_OP_DENSITY_Z && k == 0) ||
+                const bool ok_op = (pr.op == MDGPU_OP_RDF && k < 2) || (pr.op == MDGPU_OP_SDF && k == 1) || (pr.is_density() && k == 0) ||
                                    ((pr.op == MDGPU_OP_DISTANCE || pr.op == MDGPU_OP_ANGLE || pr.op == MDGPU_OP_DIHEDRAL) && !d.num_structures) || (pr.op == MDGPU_OP_COM && k == 0) ||
                                    ((pr.op == MDGPU_OP_DISTANCE_MIN || pr.op == MDGPU_OP_DISTANCE_MAX) && k < 2);
                 if (!ok_op) return bail(MDGPU_ERR_UNSUPPORTED, "property '" + pr.name + "': a dynamic selection is not lowered as argument " + std::to_string(k) + " of this procedure");
                 if (da[k].radius_min < 0.0f || da[k].radius_max < da[k].radius_min) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': The supplied radius range is invalid");   // :2654
                 pr.dyn[k].on = true; pr.dyn[k].rmin = da[k].radius_min; pr.dyn[k].rmax = da[k].radius_max;
-                if (da[k].has_and) {
-                    std::vector<uint8_t> m(sys->num_atoms, 0);
-                    for (size_t j = 0; j < da[k].and_count; ++j) { const int32_t a = da[k].and_idx[j]; if (a < 0 || (size_t)a >= sys->num_atoms) return bail(MDGPU_ERR_INVALID_ARG, "property '" + pr.name + "': atom index out of range"); m[(size_t)a] = 1; }
-                    if (pr.dyn[k].d_and_mask.upload(m.data(), m.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (selection mask)");
-                }
+                if (da[k].has_and && !take_and_mask(pr, pr.dyn[k].d_and_mask, da[k].and_idx, da[k].and_count)) return nullptr;
             }
         }
-        if (pr.op == MDGPU_OP_WITHIN_COUNT && (d.com_args & 1u)) {   // idx[2] = static side of `sel and within(...)`
-            std::vector<uint8_t> m(sys->num_atoms, 0); for (int32_t a : pr.h_idx[2]) m[(size_t)a] = 1;
-            if (pr.d_and_mask.upload(m.data(), m.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (selection mask)");
-        }
+        if (pr.op == MDGPU_OP_WITHIN_COUNT && (d.com_args & 1u) && !take_and_mask(pr, pr.d_and_mask, pr.h_idx[2].data(), pr.h_idx[2].size())) return nullptr;   // idx[2] = static side of `sel and within(...)`
         cudaError_t e = cudaSuccess;
         switch (pr.op) {
         case MDGPU_OP_RDF:
             if (pr.h_idx[0].empty() && !pr.dyn[0].on) return bail(MDGPU_ERR_INVALID_ARG, "rdf '" + pr.name + "': empty reference positions");   // internal_rdf :5396-5403
             if (pr.h_idx[1].empty() && !pr.dyn[1].on) return bail(MDGPU_ERR_INVALID_ARG, "rdf '" + pr.name + "': empty target positions");
             if (pr.cutoff_min < 0.0f || pr.cutoff_max <= pr.cutoff_min) return bail(MDGPU_ERR_INVALID_ARG, "rdf '" + pr.name + "': Invalid cutoff");
-            pr.ref_within = pr.dyn[0].on ? pr.dyn[0].rmax : 0.0f; pr.ref_within_min = pr.dyn[0].rmin;
             if (d.ref_within_radius < 0.0f || (pr.dyn[0].on && pr.n_struct) || d.ref_within_min < 0.0f) return bail(MDGPU_ERR_INVALID_ARG, "rdf '" + pr.name + "': invalid within() reference");
             if (pr.n_struct) {   // references = centres of mass of atom groups, a group's own atoms excluded (compute_rdf :5274-5275)
                 const std::string er = take_structures(pr, d, "rdf '" + pr.name + "'"); if (!er.empty()) return bail(MDGPU_ERR_INVALID_ARG, er);
                 if (pr.d_soff.upload(pr.h_soff.data(), pr.h_soff.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (structure offsets)");
             }
             if (d.num_structures_b) {   // targets = centres of mass of atom groups (coordinate_extract :1503 -> extract_com :857 on an array of selections, compute_rdf :5293-5302)
-                const size_t n = d.num_structures_b; const uint32_t* off = d.structure_offsets_b;
-                if (pr.dyn[1].on) return bail(MDGPU_ERR_INVALID_ARG, "rdf '" + pr.name + "': an array of selections cannot be a dynamic target");
-                const std::string er = check_offsets(off, n, pr.h_idx[1].size(), "rdf '" + pr.name + "'", "target group offsets", "idx[1]"); if (!er.empty()) return bail(MDGPU_ERR_INVALID_ARG, er);
-                pr.h_goff[1].assign(off, off + n + 1); pr.trg_groups = n;
-                if (pr.d_goff[1].upload(pr.h_goff[1].data(), pr.h_goff[1].size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (target group offsets)");
+                std::string er; const int code = take_group(pr, 1, d.structure_offsets_b, d.num_structures_b, "rdf '" + pr.name + "'", "target", "target group offsets", "idx[1]", er);
+                if (code) return bail(code, er);
+                pr.trg_groups = d.num_structures_b;
             }
             e = pr.d_acc.alloc(MDGPU_DIST_BINS);
             if (e == cudaSuccess) e = pr.d_frame_total.alloc(num_frames);
@@ -650,12 +660,12 @@ mdgpu_plan* mdgpu_plan_create(const mdgpu_system_desc_t* sys, const mdgpu_proper
             std::vector<uint32_t> set_of(pr.h_idx[0].size());
             for (size_t k = 0; k < pr.n_struct; ++k) for (uint32_t j = pr.h_soff[k]; j < pr.h_soff[k + 1]; ++j) set_of[j] = (uint32_t)k;
             // exclusion lists (A_i & B grown along the bonds, md_util_mask_grow_by_bonds): CSR in idx[2] / structure_offsets_b, empty when absent
-            pr.h_goff[1].assign(pr.n_struct + 1, 0u);
+            std::vector<uint32_t> excl_off(pr.n_struct + 1, 0u);
             if (d.structure_offsets_b) { if (d.num_structures_b != pr.n_struct || d.structure_offsets_b[0] != 0 || d.structure_offsets_b[pr.n_struct] != pr.h_idx[2].size()) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': exclusion offsets do not cover idx[2]");
-                                         pr.h_goff[1].assign(d.structure_offsets_b, d.structure_offsets_b + pr.n_struct + 1); }
+                                         excl_off.assign(d.structure_offsets_b, d.structure_offsets_b + pr.n_struct + 1); }
             else if (!pr.h_idx[2].empty()) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': exclusion atoms without offsets");
             e = pr.d_set_of.upload(set_of.data(), set_of.size());
-            if (e == cudaSuccess) e = pr.d_goff[1].upload(pr.h_goff[1].data(), pr.h_goff[1].size());
+            if (e == cudaSuccess) e = pr.d_excl_off.upload(excl_off.data(), excl_off.size());
             if (e == cudaSuccess) e = set_temporal(pr, num_frames, pr.n_struct);
             break; }
         case MDGPU_OP_BACKBONE_ANGLES: {   // two `dihedral in context` values per segment: phi = (C', N, CA, C), psi = (N, CA, C, N')
@@ -670,8 +680,8 @@ mdgpu_plan* mdgpu_plan_create(const mdgpu_system_desc_t* sys, const mdgpu_proper
                 for (int k = 0; k < 4; ++k) { ctx[k][2 * i] = ok ? q[k] : -1; ctx[k][2 * i + 1] = ok ? q[k + 1] : -1; }
             }
             for (int k = 0; k < 4; ++k) {
-                pr.d_idx[k].reset(); pr.h_idx[k] = ctx[k];
-                if (pr.d_idx[k].upload(pr.h_idx[k].data(), pr.h_idx[k].size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (indices)");
+                pr.h_idx[k] = ctx[k];
+                if (pr.d_idx[SPACE_FULL][k].upload(pr.h_idx[k].data(), pr.h_idx[k].size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (indices)");
             }
             pr.op = MDGPU_OP_DIHEDRAL; pr.n_struct = 2 * ns; pr.backbone_segments = ns;
             e = set_temporal(pr, num_frames, 2 * ns);
@@ -711,25 +721,27 @@ mdgpu_plan* mdgpu_plan_create(const mdgpu_system_desc_t* sys, const mdgpu_proper
         const char* env = getenv("MDGPU_INGEST_MODE");
         const uint32_t mode = env ? (uint32_t)atoi(env) : p->ingest_mode;
         p->compact = !all_atoms && mode == 0 && p->needed.size() * 4 <= N * 3;
+        for (auto& pr : p->props) for (int k = 0; k < 4; ++k) if (!pr.h_idx[k].empty()) pr.first[SPACE_FULL][k] = pr.h_idx[k][0];
         if (p->compact) {
+            AtomSpace& cs = p->space[SPACE_COMPACT];
             std::vector<int32_t> map(N, -1); for (size_t j = 0; j < p->needed.size(); ++j) map[(size_t)p->needed[j]] = (int32_t)j;
-            p->num_atoms_c = p->needed.size(); p->axis_stride_c = (p->num_atoms_c + 3) & ~(size_t)3;
-            std::vector<float> mc(p->num_atoms_c); for (size_t j = 0; j < mc.size(); ++j) mc[j] = p->h_mass[(size_t)p->needed[j]];
-            if (p->d_mass_c.upload(mc.data(), mc.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (masses)");
+            cs.num_atoms = p->needed.size(); cs.axis_stride = (cs.num_atoms + 3) & ~(size_t)3;
+            std::vector<float> mc(cs.num_atoms); for (size_t j = 0; j < mc.size(); ++j) mc[j] = p->h_mass[(size_t)p->needed[j]];
+            if (cs.d_mass.upload(mc.data(), mc.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (masses)");
             if (!p->h_radius.empty()) {
-                std::vector<float> rc(p->num_atoms_c); for (size_t j = 0; j < rc.size(); ++j) rc[j] = p->h_radius[(size_t)p->needed[j]];
-                if (p->d_radius_c.upload(rc.data(), rc.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (radii)");
+                std::vector<float> rc(cs.num_atoms); for (size_t j = 0; j < rc.size(); ++j) rc[j] = p->h_radius[(size_t)p->needed[j]];
+                if (cs.d_radius.upload(rc.data(), rc.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (radii)");
             }
             for (auto& pr : p->props) for (int k = 0; k < 4; ++k) if (!pr.h_idx[k].empty()) {
                 std::vector<int32_t> ci(pr.h_idx[k].size()); for (size_t j = 0; j < ci.size(); ++j) ci[j] = pr.h_idx[k][j] < 0 ? -1 : map[(size_t)pr.h_idx[k][j]];
-                pr.first_c[k] = ci[0];
-                if (pr.d_idx_c[k].upload(ci.data(), ci.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (indices)");
+                pr.first[SPACE_COMPACT][k] = ci[0];
+                if (pr.d_idx[SPACE_COMPACT][k].upload(ci.data(), ci.size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (indices)");
             }
-            if (p->d_init_c.alloc(3 * p->axis_stride_c) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (initial frame)");
+            if (cs.d_init.alloc(3 * cs.axis_stride) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (initial frame)");
         }
     }
     p->frame_mask.assign((num_frames + 63) / 64, 0);
-    if (p->d_init.alloc(3 * p->axis_stride) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (initial frame)");
+    if (full.d_init.alloc(3 * full.axis_stride) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (initial frame)");
     if (mdgpu_plan_clear(p) != 0) { destroy_plan(p); return nullptr; }
     return p;
 }
@@ -775,17 +787,17 @@ int mdgpu_plan_set_initial_frame(mdgpu_plan* p, const float* x, const float* y, 
     if (!p || !x || !y || !z || !cell) return fail(MDGPU_ERR_INVALID_ARG, "mdgpu_plan_set_initial_frame: null argument");
     if (p->multi) for (auto* q : p->multi->peers) { int rc = mdgpu_plan_set_initial_frame(q, x, y, z, cell); if (rc) return rc; }
     CUDA_TRY(cudaSetDevice(p->device));
-    CUDA_TRY(cudaMemcpy(p->d_init.get(), x, sizeof(float) * p->num_atoms, cudaMemcpyHostToDevice));
-    CUDA_TRY(cudaMemcpy(p->d_init.get() + p->axis_stride, y, sizeof(float) * p->num_atoms, cudaMemcpyHostToDevice));
-    CUDA_TRY(cudaMemcpy(p->d_init.get() + 2 * p->axis_stride, z, sizeof(float) * p->num_atoms, cudaMemcpyHostToDevice));
+    const AtomSpace& full = p->space[SPACE_FULL]; const float* src[3] = { x, y, z };
+    for (int ax = 0; ax < 3; ++ax) CUDA_TRY(cudaMemcpy(full.d_init.get() + (size_t)ax * full.axis_stride, src[ax], sizeof(float) * full.num_atoms, cudaMemcpyHostToDevice));
     if (p->compact) {
-        std::vector<float> c(3 * p->axis_stride_c, 0.0f); const float* src[3] = { x, y, z };
-        for (int ax = 0; ax < 3; ++ax) gather_axis(c.data() + (size_t)ax * p->axis_stride_c, src[ax], p->needed.data(), p->num_atoms_c);
-        CUDA_TRY(cudaMemcpy(p->d_init_c.get(), c.data(), sizeof(float) * c.size(), cudaMemcpyHostToDevice));
+        const AtomSpace& cs = p->space[SPACE_COMPACT];
+        std::vector<float> c(3 * cs.axis_stride, 0.0f);
+        for (int ax = 0; ax < 3; ++ax) gather_axis(c.data() + (size_t)ax * cs.axis_stride, src[ax], p->needed.data(), cs.num_atoms);
+        CUDA_TRY(cudaMemcpy(cs.d_init.get(), c.data(), sizeof(float) * c.size(), cudaMemcpyHostToDevice));
     }
     p->init_cell = *cell; p->have_init = true;
     for (auto& pr : p->props) {
-        if (pr.op >= MDGPU_OP_DENSITY_X && pr.op <= MDGPU_OP_DENSITY_Z) {
+        if (pr.is_density()) {
             // reference point / extent from the initial frame's unit cell (md_script_functions.inl:4871-4903, :4930-4933)
             const int axis = (int)pr.op - MDGPU_OP_DENSITY_X;
             const float A[3][3] = { { (float)cell->x, 0.f, 0.f }, { (float)cell->xy, (float)cell->y, 0.f }, { (float)cell->xz, (float)cell->yz, (float)cell->z } };
@@ -818,6 +830,16 @@ static size_t rdf_list_stride(const mdgpu_plan* p, const Prop& pr, const mdgpu_u
     return std::min<size_t>(nn, 125) * (pr.dyn[1].on ? std::max<size_t>(p->num_atoms / 4, 1024) : pr.h_idx[1].size()) + 1024;
 }
 
+// the scratch of one within() query over a selection of n_sel atoms; `list`: with the per-frame index list of a dynamic argument
+static int alloc_within(mdgpu_plan* p, WithinScratch& w, size_t n_sel, uint32_t cap, bool list) {
+    CUDA_TRY(w.d_geom.alloc(p->B)); CUDA_TRY(w.d_aabb.alloc((size_t)6 * p->B));
+    CUDA_TRY(w.trg.alloc(p->B, (uint32_t)p->num_atoms, cap));
+    CUDA_TRY(w.ref.alloc(p->B, (uint32_t)std::max<size_t>(n_sel, 1), cap));
+    CUDA_TRY(w.d_flags.alloc((size_t)p->B * p->num_atoms));
+    if (list) { CUDA_TRY(w.d_idx.alloc((size_t)p->B * p->num_atoms)); CUDA_TRY(w.d_n.alloc(p->B)); }
+    return 0;
+}
+
 // One stream slot with the scratch of every property, for cell capacity `cap`.
 static int build_slot(mdgpu_plan* p, Slot& s, const mdgpu_unitcell_t* first_cell, uint32_t cap) {
     CUDA_TRY(cudaStreamCreateWithFlags(s.stream.out(), cudaStreamNonBlocking));
@@ -830,18 +852,12 @@ static int build_slot(mdgpu_plan* p, Slot& s, const mdgpu_unitcell_t* first_cell
     s.ps.resize(p->props.size());
     for (size_t i = 0; i < p->props.size(); ++i) {
         Prop& pr = p->props[i]; PropScratch& ps = s.ps[i];
-        for (int k = 0; k < 4; ++k) if (pr.dyn[k].on) {   // the within() query of a dynamic argument: system-wide lists + marks + per-frame index list
-            auto& w = ps.dynw[k];
-            CUDA_TRY(w.d_geom.alloc(p->B)); CUDA_TRY(w.d_aabb.alloc((size_t)6 * p->B));
-            CUDA_TRY(w.trg.alloc(p->B, (uint32_t)p->num_atoms, cap));
-            CUDA_TRY(w.ref.alloc(p->B, (uint32_t)std::max<size_t>(pr.h_idx[k].size(), 1), cap));
-            CUDA_TRY(w.d_flags.alloc((size_t)p->B * p->num_atoms));
-            CUDA_TRY(w.d_idx.alloc((size_t)p->B * p->num_atoms)); CUDA_TRY(w.d_n.alloc(p->B));
-        }
+        for (int k = 0; k < 4; ++k) if (pr.dyn[k].on) { const int rc = alloc_within(p, ps.within[k], pr.h_idx[k].size(), cap, true); if (rc) return rc; }
+        // an argument that is an array of selections: one position per selection
+        for (int k = 0; k < 2; ++k) if (!pr.h_goff[k].empty()) CUDA_TRY(ps.d_gpos[k].alloc((size_t)p->B * (pr.h_goff[k].size() - 1) * 3));
         if (pr.needs_cells() && pr.share_trg < 0) {
             CUDA_TRY(ps.d_geom.alloc(p->B)); CUDA_TRY(ps.d_aabb.alloc((size_t)6 * p->B));
             CUDA_TRY(ps.trg.alloc(p->B, (uint32_t)(pr.dyn[1].on ? p->num_atoms : (pr.trg_groups ? pr.trg_groups : pr.h_idx[1].size())), cap));
-            if (pr.trg_groups) CUDA_TRY(ps.d_gpos[1].alloc((size_t)p->B * pr.trg_groups * 3));
         }
         if (pr.op == MDGPU_OP_RDF) {
             CUDA_TRY(ps.ref.alloc(p->B, (uint32_t)(pr.dyn[0].on ? p->num_atoms : (pr.n_struct ? pr.n_struct : pr.h_idx[0].size())), cap));
@@ -859,14 +875,8 @@ static int build_slot(mdgpu_plan* p, Slot& s, const mdgpu_unitcell_t* first_cell
             CUDA_TRY(ps.d_sdf_xyzw.alloc((size_t)p->B * (pr.n_struct + 1) * pr.struct_size));
             CUDA_TRY(ps.d_sdf_ref0.alloc((size_t)p->B * 20));
             CUDA_TRY(ps.d_sdf_mats.alloc((size_t)p->B * pr.n_struct * 32));
-        } else if (pr.op == MDGPU_OP_DISTANCE_PAIR || ((pr.op == MDGPU_OP_DISTANCE_MIN || pr.op == MDGPU_OP_DISTANCE_MAX || (pr.op >= MDGPU_OP_COORD_X && pr.op <= MDGPU_OP_COORD_Z) || pr.op == MDGPU_OP_PLANE) && (!pr.h_goff[0].empty() || !pr.h_goff[1].empty()))) {
-            for (int k = 0; k < 2; ++k) if (!pr.h_goff[k].empty()) CUDA_TRY(ps.d_gpos[k].alloc((size_t)p->B * (pr.h_goff[k].size() - 1) * 3));
-            if (pr.op == MDGPU_OP_PLANE) CUDA_TRY(ps.d_sdf_xyzw.alloc((size_t)p->B * pr.h_idx[0].size()));   // the plane fit's xyzw scratch
         } else if (pr.op == MDGPU_OP_WITHIN_COUNT) {
-            CUDA_TRY(ps.d_geom.alloc(p->B)); CUDA_TRY(ps.d_aabb.alloc((size_t)6 * p->B));
-            CUDA_TRY(ps.trg.alloc(p->B, (uint32_t)p->num_atoms, cap));
-            CUDA_TRY(ps.ref.alloc(p->B, (uint32_t)std::max<size_t>(pr.h_idx[0].size(), 1), cap));
-            CUDA_TRY(ps.d_flags.alloc((size_t)p->B * p->num_atoms));
+            const int rc = alloc_within(p, ps.within[0], pr.h_idx[0].size(), cap, false); if (rc) return rc;
         } else if (pr.op == MDGPU_OP_POROSITY) {
             CUDA_TRY(ps.d_poro_xyzr.alloc((size_t)PORO_FRAMES * pr.h_idx[0].size())); CUDA_TRY(ps.d_poro_hdr.alloc(PORO_FRAMES));
             CUDA_TRY(ps.d_poro_grid.alloc((size_t)PORO_FRAMES * PORO_GRID_WORDS)); CUDA_TRY(ps.d_poro_count.alloc(PORO_FRAMES));
@@ -875,8 +885,8 @@ static int build_slot(mdgpu_plan* p, Slot& s, const mdgpu_unitcell_t* first_cell
         } else if (pr.op == MDGPU_OP_RMSD) {
             CUDA_TRY(ps.d_sdf_xyzw.alloc((size_t)p->B * 2 * pr.h_idx[0].size()));   // [B][initial, current][atoms]
         } else if (pr.op == MDGPU_OP_PLANE || pr.op == MDGPU_OP_SHAPE_WEIGHTS) {
-            CUDA_TRY(ps.d_sdf_xyzw.alloc((size_t)p->B * pr.h_idx[0].size()));
-        } else if (pr.op >= MDGPU_OP_DENSITY_X && pr.op <= MDGPU_OP_DENSITY_Z) {
+            CUDA_TRY(ps.d_sdf_xyzw.alloc((size_t)p->B * pr.h_idx[0].size()));   // the fit's xyzw scratch
+        } else if (pr.is_density()) {
             CUDA_TRY(ps.d_frame_bins64.alloc((size_t)p->B * MDGPU_DIST_BINS));
         } else if (pr.com_mask) {
             if (!pr.n_struct) CUDA_TRY(ps.d_argpos.alloc((size_t)p->B * 12));
@@ -896,13 +906,14 @@ static int ensure_slots(mdgpu_plan* p, const mdgpu_unitcell_t* first_cell, bool 
         uint32_t cap = p->cell_cap;
         if (!cap) {
             uint64_t need = 1u << 16;   // floor: non-periodic axes get their extent from the data (AABB fit), unknown here
-            for (auto& pr : p->props) if (pr.needs_cells() || pr.op == MDGPU_OP_WITHIN_COUNT) {
-                FrameGeom g; host_frame_geom(&g, first_cell, pr.op == MDGPU_OP_WITHIN_COUNT ? within_cell_ext(pr.cutoff_max) : (double)pr.cutoff_max, pr.cutoff_max, nullptr, 0xffffffffu);
+            auto grid = [&](double cell_ext, float cutoff) {
+                FrameGeom g; host_frame_geom(&g, first_cell, cell_ext, cutoff, nullptr, 0xffffffffu);
                 need = std::max<uint64_t>(need, 2ull * std::max<uint64_t>(g.num_cells, g.num_home) + 2);
-            }
-            for (auto& pr : p->props) for (auto& dy : pr.dyn) if (dy.on) {
-                FrameGeom g; host_frame_geom(&g, first_cell, within_cell_ext(dy.rmax), dy.rmax, nullptr, 0xffffffffu);
-                need = std::max<uint64_t>(need, 2ull * std::max<uint64_t>(g.num_cells, g.num_home) + 2);
+            };
+            for (auto& pr : p->props) {
+                if (pr.needs_cells()) grid((double)pr.cutoff_max, pr.cutoff_max);
+                if (pr.op == MDGPU_OP_WITHIN_COUNT) grid(within_cell_ext(pr.cutoff_max), pr.cutoff_max);
+                for (auto& dy : pr.dyn) if (dy.on) grid(within_cell_ext(dy.rmax), dy.rmax);
             }
             cap = (uint32_t)std::min<uint64_t>(need, 1u << 26);
         }
@@ -911,7 +922,7 @@ static int ensure_slots(mdgpu_plan* p, const mdgpu_unitcell_t* first_cell, bool 
         p->slots = std::move(slots); p->cell_cap = cap;
     }
     if (need_host_staging) for (auto& s : p->slots) if (!s.d_frames.get()) {   // host ingest staging, in the ingest (compact or full) atom space
-        const size_t n = (size_t)p->B * 3 * (p->compact ? p->axis_stride_c : p->axis_stride);
+        const size_t n = (size_t)p->B * 3 * p->space[p->ingest_space()].axis_stride;
         DevBuf<float> d; PinnedBuf<float> h;
         CUDA_TRY(d.alloc(n));
         CUDA_TRY(h.alloc(n));
@@ -920,9 +931,6 @@ static int ensure_slots(mdgpu_plan* p, const mdgpu_unitcell_t* first_cell, bool 
     return 0;
 }
 
-// enqueue the property kernels of one batch whose frames are already in device memory
-// `c`: the frames are in the plan's COMPACT atom space (host ingest copied only the atoms the properties read): index lists, masses and the
-// initial frame of that space are used; otherwise the caller's full frames with global atom indices.
 // position of argument k of distance / angle / dihedral / com when it is a selection: its centre of mass (coordinate_extract_com
 // md_script_functions.inl:1717), or for an array of selections the centre of the selections' centres (:1826-1842) -> ps.d_argpos[f][k]
 static void arg_position(Prop& pr, PropScratch& ps, int k, const BatchFrames& fr, Slot& s, int32_t* const* didx, const float* dmass, DynSel dsel) {
@@ -933,9 +941,46 @@ static void arg_position(Prop& pr, PropScratch& ps, int k, const BatchFrames& fr
     } else launch_arg_com(fr, s.d_cells.get(), didx[k], (uint32_t)pr.h_idx[k].size(), dmass, ps.d_argpos.get(), k, s.stream, dsel);
 }
 
-static int enqueue_batch(mdgpu_plan* p, Slot& s, const BatchFrames& fr, uint32_t frame0, bool c) {
+// Argument k as positions: an array of selections contributes one position per selection, its centre of mass (extract_com :857, no periodic
+// treatment; coordinate_extract :1503) -> ps.d_gpos[k]; any other argument is the atoms of idx[k] (pos == null)
+struct ArgPoints { uint32_t n; const float* pos; };
+static ArgPoints group_positions(Prop& pr, PropScratch& ps, int k, const BatchFrames& fr, const int32_t* didx, const float* dmass, cudaStream_t st) {
+    if (pr.h_goff[k].empty()) return ArgPoints{ (uint32_t)pr.h_idx[k].size(), nullptr };
+    const uint32_t n = (uint32_t)pr.h_goff[k].size() - 1;
+    launch_group_com(fr, didx, pr.d_goff[k].get(), n, dmass, ps.d_gpos[k].get(), st);
+    return ArgPoints{ n, ps.d_gpos[k].get() };
+}
+
+// within([rmin:]rmax, sel) of every frame of the batch up to the marking kernel: the grid over every atom of the system (get_spatial_acc :734),
+// the cell lists of all atoms and of the selection, and the arguments of launch_within_count / launch_within_list (`out` is the caller's)
+static WithinArgs enqueue_within(mdgpu_plan* p, Slot& s, WithinScratch& w, const BatchFrames& fr, bool all_pbc, const int32_t* sel, size_t n_sel, float rmin, float rmax, const uint8_t* and_mask, uint32_t frame0) {
+    const float* aabb = nullptr;
+    if (!all_pbc) { launch_aabb(fr, nullptr, (uint32_t)p->num_atoms, w.d_aabb.get(), s.stream); aabb = w.d_aabb.get(); }
+    launch_geom(s.d_cells.get(), aabb, w.d_geom.get(), within_cell_ext(rmax), (double)rmax, p->cell_cap, (int)fr.count, s.d_err.get(), s.stream);
+    launch_cell_list(0, fr, nullptr, nullptr, (uint32_t)p->num_atoms, w.d_geom.get(), w.trg.cl, 0, s.stream);
+    launch_cell_list(1, fr, sel, nullptr, (uint32_t)n_sel, w.d_geom.get(), w.ref.cl, 0, s.stream);
+    WithinArgs a{};
+    a.geom = w.d_geom.get(); a.trg = w.trg.cl; a.ref = w.ref.cl; a.sel = sel; a.n_sel = (uint32_t)n_sel;
+    a.num_atoms = (uint32_t)p->num_atoms; a.flags = w.d_flags.get(); a.out = nullptr; a.frame0 = frame0; a.min_r2 = rmin * rmin; a.and_mask = and_mask;   // :2641
+    return a;
+}
+
+// what `launch` enqueues on `st`, timed as one TimedLaunch of `kind` when kernel timing is enabled
+template <typename F> static void timed_launch(mdgpu_plan* p, cudaStream_t st, int kind, F&& launch) {
+    TimedLaunch tl{ nullptr, nullptr, kind };
+    if (p->timing) { cudaEventCreate(&tl.a); cudaEventCreate(&tl.b); cudaEventRecord(tl.a, st); }
+    launch();
+    if (p->timing) { cudaEventRecord(tl.b, st); p->timed.push_back(tl); }
+}
+
+// enqueue the property kernels of one batch whose frames are already in device memory, in atom space `sp`: SPACE_COMPACT when host ingest
+// copied only the atoms the properties read (index lists, masses and the initial frame of that space are used), SPACE_FULL for whole frames
+// with global atom indices.
+static int enqueue_batch(mdgpu_plan* p, Slot& s, const BatchFrames& fr, uint32_t frame0, Space sp) {
     std::lock_guard<std::mutex> guard(p->submit_mutex);
     const int B = (int)fr.count;
+    const AtomSpace& as = p->space[sp];
+    const float* dmass = as.d_mass.get(); const float* dinit = as.d_init.get(); const size_t init_as = as.axis_stride;
     // all frames of a batch must agree on ortho vs triclinic (kernel template parameter)
     bool tri = (s.h_cells[0].flags & MDGPU_CELL_TRICLINIC) != 0;
     for (int i = 1; i < B; ++i) if (((s.h_cells[i].flags & MDGPU_CELL_TRICLINIC) != 0) != tri)
@@ -944,37 +989,26 @@ static int enqueue_batch(mdgpu_plan* p, Slot& s, const BatchFrames& fr, uint32_t
     bool all_pbc = true; for (int i = 0; i < B; ++i) all_pbc = all_pbc && ((s.h_cells[i].flags & MDGPU_CELL_PBC_ALL) == MDGPU_CELL_PBC_ALL);
     for (size_t i = 0; i < p->props.size(); ++i) {
         Prop& pr = p->props[i]; PropScratch& ps = s.ps[i];
-        int32_t* didx[4]; for (int k = 0; k < 4; ++k) didx[k] = (c ? pr.d_idx_c[k] : pr.d_idx[k]).get();
-        const float* dmass = c ? p->d_mass_c.get() : p->d_mass.get(); const float* dinit = c ? p->d_init_c.get() : p->d_init.get(); const size_t init_as = c ? p->axis_stride_c : p->axis_stride;
+        int32_t* didx[4]; for (int k = 0; k < 4; ++k) didx[k] = pr.d_idx[sp][k].get();
         const PropScratch& cs = (pr.share_trg >= 0) ? s.ps[pr.share_trg] : ps;   // owner of the target cell list + geometry
         DynSel dsel[4];
         for (int k = 0; k < 4; ++k) {   // dynamic arguments first: within([min:]max, idx[k]) [and mask] of every frame of the batch -> ascending per-frame lists
             dsel[k] = DynSel{ nullptr, nullptr, 0 };
             if (!pr.dyn[k].on) continue;
-            auto& w = ps.dynw[k];
-            const float* waabb = nullptr;
-            if (!all_pbc) { launch_aabb(fr, nullptr, (uint32_t)p->num_atoms, w.d_aabb.get(), s.stream); waabb = w.d_aabb.get(); }   // every atom of the system (get_spatial_acc :734)
-            launch_geom(s.d_cells.get(), waabb, w.d_geom.get(), within_cell_ext(pr.dyn[k].rmax), (double)pr.dyn[k].rmax, p->cell_cap, B, s.d_err.get(), s.stream);
-            launch_cell_list(0, fr, nullptr, nullptr, (uint32_t)p->num_atoms, w.d_geom.get(), w.trg.cl, 0, s.stream);
-            launch_cell_list(1, fr, didx[k], nullptr, (uint32_t)pr.h_idx[k].size(), w.d_geom.get(), w.ref.cl, 0, s.stream);
-            WithinArgs wa{};
-            wa.geom = w.d_geom.get(); wa.trg = w.trg.cl; wa.ref = w.ref.cl; wa.sel = didx[k]; wa.n_sel = (uint32_t)pr.h_idx[k].size();
-            wa.num_atoms = (uint32_t)p->num_atoms; wa.flags = w.d_flags.get(); wa.out = nullptr; wa.frame0 = frame0; wa.min_r2 = pr.dyn[k].rmin * pr.dyn[k].rmin; wa.and_mask = pr.dyn[k].d_and_mask.get();
+            auto& w = ps.within[k];
+            const WithinArgs wa = enqueue_within(p, s, w, fr, all_pbc, didx[k], pr.h_idx[k].size(), pr.dyn[k].rmin, pr.dyn[k].rmax, pr.dyn[k].d_and_mask.get(), frame0);
             launch_within_list(wa, B, tri, p->sm_count, w.d_idx.get(), w.d_n.get(), s.stream);
             dsel[k] = DynSel{ w.d_idx.get(), w.d_n.get(), (uint32_t)p->num_atoms };
         }
         if (pr.needs_cells() && pr.share_trg < 0) {
+            // target groups: the target points are the groups' centres of mass, an AoS stream, j = position index (compute_rdf :5299-5301);
+            // otherwise the atoms of idx[1], or of the frame's dynamic selection (an array of selections is never dynamic: dsel[1] is empty then)
+            const ArgPoints t = group_positions(pr, ps, 1, fr, didx[1], dmass, s.stream);
+            const int32_t* tidx = t.pos ? nullptr : didx[1];
             const float* aabb = nullptr;
-            if (pr.trg_groups) {   // the target points are the groups' centres of mass: an AoS stream, j = position index (compute_rdf :5299-5301)
-                launch_group_com(fr, didx[1], pr.d_goff[1].get(), (uint32_t)pr.trg_groups, dmass, ps.d_gpos[1].get(), s.stream);
-                if (!all_pbc) { launch_aabb(fr, nullptr, (uint32_t)pr.trg_groups, ps.d_aabb.get(), s.stream, DynSel{ nullptr, nullptr, 0 }, ps.d_gpos[1].get()); aabb = ps.d_aabb.get(); }
-                launch_geom(s.d_cells.get(), aabb, ps.d_geom.get(), (double)pr.cutoff_max, (double)pr.cutoff_max, p->cell_cap, B, s.d_err.get(), s.stream);
-                launch_cell_list(0, fr, nullptr, ps.d_gpos[1].get(), (uint32_t)pr.trg_groups, ps.d_geom.get(), ps.trg.cl, 0, s.stream);
-            } else {
-            if (!all_pbc) { launch_aabb(fr, didx[1], (uint32_t)pr.h_idx[1].size(), ps.d_aabb.get(), s.stream, dsel[1]); aabb = ps.d_aabb.get(); }
+            if (!all_pbc) { launch_aabb(fr, tidx, t.n, ps.d_aabb.get(), s.stream, dsel[1], t.pos); aabb = ps.d_aabb.get(); }
             launch_geom(s.d_cells.get(), aabb, ps.d_geom.get(), (double)pr.cutoff_max, (double)pr.cutoff_max, p->cell_cap, B, s.d_err.get(), s.stream);
-            launch_cell_list(0, fr, didx[1], nullptr, (uint32_t)pr.h_idx[1].size(), ps.d_geom.get(), ps.trg.cl, 0, s.stream, dsel[1]);
-            }
+            launch_cell_list(0, fr, tidx, t.pos, t.n, ps.d_geom.get(), ps.trg.cl, 0, s.stream, dsel[1]);
         }
         switch (pr.op) {
         case MDGPU_OP_RDF: {
@@ -1021,7 +1055,7 @@ static int enqueue_batch(mdgpu_plan* p, Slot& s, const BatchFrames& fr, uint32_t
             a.geom = cs.d_geom.get(); a.trg = cs.trg.cl; a.ref = ps.ref.cl;
             a.inv_cutoff_range = 1.0f; a.min_cutoff = 0.0f; a.min_r2 = 0.0f;
             a.frame_bins = ps.d_frame_bins.get(); a.frame0 = frame0; a.err = s.d_err.get();
-            a.excl_off = pr.d_goff[1].get(); a.excl_idx = didx[2]; a.ref_set = pr.d_set_of.get(); a.count_mode = 1;
+            a.excl_off = pr.d_excl_off.get(); a.excl_idx = didx[2]; a.ref_set = pr.d_set_of.get(); a.count_mode = 1;
             launch_rdf(a, B, tri, 1, p->sm_count, s.stream, nullptr);
             launch_contact_rows(ps.d_frame_bins.get(), (uint32_t)pr.n_struct, pr.d_temporal.get(), frame0, B, s.stream);
             break; }
@@ -1034,10 +1068,7 @@ static int enqueue_batch(mdgpu_plan* p, Slot& s, const BatchFrames& fr, uint32_t
             a.unwrap_pairs = pr.d_unwrap.get(); a.n_unwrap = pr.n_unwrap; a.cutoff = pr.cutoff_max;
             a.scratch_xyzw = ps.d_sdf_xyzw.get(); a.ref0 = ps.d_sdf_ref0.get(); a.matrices = ps.d_sdf_mats.get();
             a.vol = pr.d_vol.get(); a.frame_total = pr.d_frame_total.get(); a.frame0 = frame0;
-            TimedLaunch tl{};
-            if (p->timing) { cudaEventCreate(&tl.a); cudaEventCreate(&tl.b); cudaEventRecord(tl.a, s.stream); }
-            launch_sdf(a, B, tri, s.stream);
-            if (p->timing) { cudaEventRecord(tl.b, s.stream); tl.kind = 1; p->timed.push_back(tl); }
+            timed_launch(p, s.stream, 1, [&] { launch_sdf(a, B, tri, s.stream); });
             break; }
         case MDGPU_OP_DENSITY_X: case MDGPU_OP_DENSITY_Y: case MDGPU_OP_DENSITY_Z: {
             if (!p->have_init) return fail(MDGPU_ERR_INVALID_ARG, "density '%s' needs the initial frame (mdgpu_plan_set_initial_frame)", pr.name.c_str());
@@ -1045,38 +1076,25 @@ static int enqueue_batch(mdgpu_plan* p, Slot& s, const BatchFrames& fr, uint32_t
             a.frames = fr; a.idx = didx[0]; a.n = (uint32_t)pr.h_idx[0].size(); a.mass = dmass; a.axis = (int)pr.op - MDGPU_OP_DENSITY_X; a.dyn = dsel[0];
             a.rc = pr.rc; a.re = pr.re; a.inv_ext = pr.inv_ext; a.min_point = pr.min_point;
             a.acc = pr.d_acc.get(); a.frame_bins = ps.d_frame_bins64.get(); a.frame_min = pr.d_frame_min64.get(); a.frame_max = pr.d_frame_max64.get(); a.keep = pr.d_keep64.get(); a.frame0 = frame0;
-            TimedLaunch tl{};
-            if (p->timing) { cudaEventCreate(&tl.a); cudaEventCreate(&tl.b); cudaEventRecord(tl.a, s.stream); }
-            launch_density(a, B, s.stream);
-            if (p->timing) { cudaEventRecord(tl.b, s.stream); tl.kind = 2; p->timed.push_back(tl); }
+            timed_launch(p, s.stream, 2, [&] { launch_density(a, B, s.stream); });
             break; }
         case MDGPU_OP_WITHIN_COUNT: {
-            const float* aabb = nullptr;
-            if (!all_pbc) { launch_aabb(fr, nullptr, (uint32_t)p->num_atoms, ps.d_aabb.get(), s.stream); aabb = ps.d_aabb.get(); }   // every atom of the system
-            launch_geom(s.d_cells.get(), aabb, ps.d_geom.get(), within_cell_ext(pr.cutoff_max), (double)pr.cutoff_max, p->cell_cap, B, s.d_err.get(), s.stream);
-            launch_cell_list(0, fr, nullptr, nullptr, (uint32_t)p->num_atoms, ps.d_geom.get(), ps.trg.cl, 0, s.stream);
-            launch_cell_list(1, fr, didx[0], nullptr, (uint32_t)pr.h_idx[0].size(), ps.d_geom.get(), ps.ref.cl, 0, s.stream);
-            WithinArgs a{};
-            a.geom = ps.d_geom.get(); a.trg = ps.trg.cl; a.ref = ps.ref.cl; a.sel = didx[0]; a.n_sel = (uint32_t)pr.h_idx[0].size();
-            a.num_atoms = (uint32_t)p->num_atoms; a.flags = ps.d_flags.get(); a.out = pr.d_temporal.get(); a.frame0 = frame0; a.min_r2 = pr.cutoff_min * pr.cutoff_min; a.and_mask = pr.d_and_mask.get();   // :2641
+            WithinArgs a = enqueue_within(p, s, ps.within[0], fr, all_pbc, didx[0], pr.h_idx[0].size(), pr.cutoff_min, pr.cutoff_max, pr.d_and_mask.get(), frame0);
+            a.out = pr.d_temporal.get();
             launch_within_count(a, B, tri, p->sm_count, s.stream);
             break; }
         case MDGPU_OP_COM: {
             TemporalArgs a{};
             a.frames = fr; a.cells = s.d_cells.get(); a.op = (int)pr.op; a.out = pr.d_temporal.get(); a.frame0 = frame0;
-            a.atom[0] = c ? pr.first_c[0] : pr.h_idx[0][0]; a.pos = ps.d_argpos.get(); a.com_mask = pr.com_mask;
+            a.atom[0] = pr.first[sp][0]; a.pos = ps.d_argpos.get(); a.com_mask = pr.com_mask;
             if (pr.com_mask & 1u) arg_position(pr, ps, 0, fr, s, didx, dmass, dsel[0]);
             launch_com_rows(a, B, s.stream);
             break; }
-        case MDGPU_OP_COORD_X: case MDGPU_OP_COORD_Y: case MDGPU_OP_COORD_Z:
-            if (!pr.h_goff[0].empty()) {
-                const uint32_t n = (uint32_t)pr.h_goff[0].size() - 1;
-                launch_group_com(fr, didx[0], pr.d_goff[0].get(), n, dmass, ps.d_gpos[0].get(), s.stream);
-                launch_coord_rows_pos(ps.d_gpos[0].get(), n, (int)pr.op - MDGPU_OP_COORD_X, pr.d_temporal.get(), frame0, B, s.stream);
-                break;
-            }
-            launch_coord_rows(fr, didx[0], (uint32_t)pr.h_idx[0].size(), (int)pr.op - MDGPU_OP_COORD_X, pr.d_temporal.get(), frame0, s.stream);
-            break;
+        case MDGPU_OP_COORD_X: case MDGPU_OP_COORD_Y: case MDGPU_OP_COORD_Z: {
+            const ArgPoints g = group_positions(pr, ps, 0, fr, didx[0], dmass, s.stream);
+            if (g.pos) launch_coord_rows_pos(g.pos, g.n, (int)pr.op - MDGPU_OP_COORD_X, pr.d_temporal.get(), frame0, B, s.stream);
+            else launch_coord_rows(fr, didx[0], g.n, (int)pr.op - MDGPU_OP_COORD_X, pr.d_temporal.get(), frame0, s.stream);
+            break; }
         case MDGPU_OP_SHAPE_WEIGHTS: {
             ShapeArgs a{};
             a.frames = fr; a.cells = s.d_cells.get(); a.mass = dmass; a.use_mass = (int)(pr.com_mask & 1u);
@@ -1086,28 +1104,21 @@ static int enqueue_batch(mdgpu_plan* p, Slot& s, const BatchFrames& fr, uint32_t
             break; }
         case MDGPU_OP_PLANE: {
             RmsdArgs a{};
-            a.frames = fr; a.cells = s.d_cells.get(); a.mass = dmass; a.idx = didx[0]; a.n = (uint32_t)pr.h_idx[0].size();
-            if (!pr.h_goff[0].empty()) {
-                a.n = (uint32_t)pr.h_goff[0].size() - 1;
-                launch_group_com(fr, didx[0], pr.d_goff[0].get(), a.n, dmass, ps.d_gpos[0].get(), s.stream); a.pos = ps.d_gpos[0].get();
-            }
+            const ArgPoints g = group_positions(pr, ps, 0, fr, didx[0], dmass, s.stream);
+            a.frames = fr; a.cells = s.d_cells.get(); a.mass = dmass; a.idx = didx[0]; a.n = g.n; a.pos = g.pos;
             a.unwrap_pairs = pr.d_unwrap.get(); a.n_unwrap = pr.n_unwrap; a.scratch_xyzw = ps.d_sdf_xyzw.get(); a.out = pr.d_temporal.get(); a.frame0 = frame0;
             launch_plane(a, B, s.stream);
             break; }
         case MDGPU_OP_DISTANCE_PAIR: {
-            uint32_t cnt[2];
-            for (int k = 0; k < 2; ++k) {
-                cnt[k] = (uint32_t)(pr.h_goff[k].empty() ? pr.h_idx[k].size() : pr.h_goff[k].size() - 1);
-                if (!pr.h_goff[k].empty()) launch_group_com(fr, didx[k], pr.d_goff[k].get(), cnt[k], dmass, ps.d_gpos[k].get(), s.stream);   // extract_com :857, as for rdf's group references
-            }
-            launch_distance_pair(fr, s.d_cells.get(), didx[0], cnt[0], didx[1], cnt[1], ps.d_gpos[0].get(), ps.d_gpos[1].get(), pr.d_temporal.get(), frame0, s.stream);
+            const ArgPoints g0 = group_positions(pr, ps, 0, fr, didx[0], dmass, s.stream), g1 = group_positions(pr, ps, 1, fr, didx[1], dmass, s.stream);
+            launch_distance_pair(fr, s.d_cells.get(), didx[0], g0.n, didx[1], g1.n, g0.pos, g1.pos, pr.d_temporal.get(), frame0, s.stream);
             break; }
         case MDGPU_OP_POROSITY:   // sub-batches of PORO_FRAMES frames through the slot's grids
             for (uint32_t f0 = 0; f0 < (uint32_t)B; f0 += PORO_FRAMES) {
                 const uint32_t nf = std::min<uint32_t>(PORO_FRAMES, (uint32_t)B - f0);
                 PorosityArgs a{};
                 a.frames = BatchFrames{ fr.xyz + (size_t)f0 * fr.frame_stride, fr.frame_stride, fr.axis_stride, nf }; a.cells = s.d_cells.get() + f0;
-                a.idx = didx[0]; a.n = (uint32_t)pr.h_idx[0].size(); a.radius = c ? p->d_radius_c.get() : p->d_radius.get();
+                a.idx = didx[0]; a.n = (uint32_t)pr.h_idx[0].size(); a.radius = as.d_radius.get();
                 a.xyzr = ps.d_poro_xyzr.get(); a.hdr = ps.d_poro_hdr.get(); a.grid = ps.d_poro_grid.get(); a.count = ps.d_poro_count.get();
                 a.frame_set = pr.d_frame_total.get(); a.frame_n = pr.d_frame_n.get(); a.out = pr.d_temporal.get(); a.frame0 = frame0 + f0;
                 launch_porosity(a, (int)nf, s.stream);
@@ -1121,18 +1132,11 @@ static int enqueue_batch(mdgpu_plan* p, Slot& s, const BatchFrames& fr, uint32_t
             a.scratch_xyzw = ps.d_sdf_xyzw.get(); a.out = pr.d_temporal.get(); a.frame0 = frame0;
             launch_rmsd(a, B, s.stream);
             break; }
-        case MDGPU_OP_DISTANCE_MIN: case MDGPU_OP_DISTANCE_MAX:   // both evaluate md_util_min_distance (md_script_functions.inl:3904, 3944)
-            if (!pr.h_goff[0].empty() || !pr.h_goff[1].empty()) {
-                uint32_t cnt[2];
-                for (int k = 0; k < 2; ++k) {
-                    cnt[k] = (uint32_t)(pr.h_goff[k].empty() ? pr.h_idx[k].size() : pr.h_goff[k].size() - 1);
-                    if (!pr.h_goff[k].empty()) launch_group_com(fr, didx[k], pr.d_goff[k].get(), cnt[k], dmass, ps.d_gpos[k].get(), s.stream);
-                }
-                launch_min_distance_pos(fr, s.d_cells.get(), didx[0], cnt[0], didx[1], cnt[1], ps.d_gpos[0].get(), ps.d_gpos[1].get(), pr.d_temporal.get(), frame0, s.stream);
-                break;
-            }
-            launch_min_distance(fr, s.d_cells.get(), didx[0], (uint32_t)pr.h_idx[0].size(), didx[1], (uint32_t)pr.h_idx[1].size(), pr.d_temporal.get(), frame0, s.stream, dsel[0], dsel[1]);
-            break;
+        case MDGPU_OP_DISTANCE_MIN: case MDGPU_OP_DISTANCE_MAX: {   // both evaluate md_util_min_distance (md_script_functions.inl:3904, 3944)
+            const ArgPoints g0 = group_positions(pr, ps, 0, fr, didx[0], dmass, s.stream), g1 = group_positions(pr, ps, 1, fr, didx[1], dmass, s.stream);
+            if (g0.pos || g1.pos) launch_min_distance_pos(fr, s.d_cells.get(), didx[0], g0.n, didx[1], g1.n, g0.pos, g1.pos, pr.d_temporal.get(), frame0, s.stream);
+            else launch_min_distance(fr, s.d_cells.get(), didx[0], g0.n, didx[1], g1.n, pr.d_temporal.get(), frame0, s.stream, dsel[0], dsel[1]);
+            break; }
         case MDGPU_OP_DISTANCE: case MDGPU_OP_ANGLE: case MDGPU_OP_DIHEDRAL: {
             TemporalArgs a{};
             a.frames = fr; a.cells = s.d_cells.get(); a.op = (int)pr.op; a.out = pr.d_temporal.get(); a.frame0 = frame0;
@@ -1148,7 +1152,7 @@ static int enqueue_batch(mdgpu_plan* p, Slot& s, const BatchFrames& fr, uint32_t
                 launch_temporal_ctx(a, B, s.stream);
                 break;
             }
-            for (int k = 0; k < 4; ++k) a.atom[k] = pr.h_idx[k].empty() ? 0 : (c ? pr.first_c[k] : pr.h_idx[k][0]);
+            for (int k = 0; k < 4; ++k) a.atom[k] = pr.first[sp][k];
             a.pos = ps.d_argpos.get(); a.com_mask = pr.com_mask;
             for (int k = 0; k < 4; ++k) if (pr.com_mask & (1u << k)) arg_position(pr, ps, k, fr, s, didx, dmass, dsel[k]);
             launch_temporal(a, B, s.stream);
@@ -1195,8 +1199,14 @@ static int retire_slot(mdgpu_plan* p, Slot& s) {
     return 0;
 }
 
-// Slot ownership: the calling thread gets exclusive use of one slot (stream + staging buffers), with that slot's previous batch retired.
-static int acquire_slot(mdgpu_plan* p, Slot** out, int want = -1) {
+// Slot ownership: the calling thread gets exclusive use of one slot (stream + staging buffers), with that slot's previous batch retired,
+// for as long as it holds the lease (move-only); the slot is handed back when the lease is destroyed or reset.
+struct SlotRelease {
+    mdgpu_plan* p = nullptr;
+    void operator()(Slot* s) const { { std::lock_guard<std::mutex> lk(p->slot_mutex); s->owned = false; } p->slot_cv.notify_all(); }
+};
+using SlotLease = std::unique_ptr<Slot, SlotRelease>;
+static int acquire_slot(mdgpu_plan* p, SlotLease& out, int want = -1) {   // the next free slot in ring order, or slot `want`: waits until it is free
     Slot* s = nullptr;
     {
         std::unique_lock<std::mutex> lk(p->slot_mutex);
@@ -1209,25 +1219,20 @@ static int acquire_slot(mdgpu_plan* p, Slot** out, int want = -1) {
         }
         s->owned = true;
     }
-    *out = s;
+    out = SlotLease(s, SlotRelease{ p });
     const int rc = retire_slot(p, *s);
-    if (rc) { std::lock_guard<std::mutex> lk(p->slot_mutex); s->owned = false; p->slot_cv.notify_all(); *out = nullptr; }
+    if (rc) out.reset();
     return rc;
-}
-static void release_slot(mdgpu_plan* p, Slot* s) {
-    if (!s) return;
-    { std::lock_guard<std::mutex> lk(p->slot_mutex); s->owned = false; }
-    p->slot_cv.notify_all();
 }
 // retire every slot (waits for all batches in flight, whoever enqueued them)
 static int drain_slots(mdgpu_plan* p) {
     int rc = 0;
-    for (size_t i = 0; i < p->slots.size(); ++i) { Slot* s = nullptr; const int r = acquire_slot(p, &s, (int)i); if (r && !rc) rc = r; release_slot(p, s); }
+    for (size_t i = 0; i < p->slots.size(); ++i) { SlotLease lease; const int r = acquire_slot(p, lease, (int)i); if (r && !rc) rc = r; }
     return rc;
 }
 
 static const mdgpu_unitcell_t* cell_at(const mdgpu_unitcell_t* cells, size_t stride_bytes, size_t i) {
-    return (const mdgpu_unitcell_t*)((const char*)cells + i * (stride_bytes ? stride_bytes : 0));
+    return (const mdgpu_unitcell_t*)((const char*)cells + i * stride_bytes);
 }
 
 static int eval_host_frames_1(mdgpu_plan* p, const float* h_xyz, size_t frame_stride, size_t axis_stride, const mdgpu_unitcell_t* cells, size_t cell_stride_bytes, uint32_t frame_beg, uint32_t count);
@@ -1348,12 +1353,10 @@ int mdgpu_eval_device_frames(mdgpu_plan* p, const float* d_xyz, size_t frame_str
     for (uint32_t b0 = 0; b0 < count; b0 += p->B) {
         if (p->interrupt.load()) return fail(MDGPU_ERR_INTERRUPTED, "evaluation interrupted");
         const uint32_t nb = std::min(p->B, count - b0);
-        Slot* s = nullptr; rc = acquire_slot(p, &s); if (rc) return rc;
+        SlotLease s; rc = acquire_slot(p, s); if (rc) return rc;
         for (uint32_t i = 0; i < nb; ++i) s->h_cells[i] = *cell_at(cells, cell_stride_bytes, b0 + i);
         BatchFrames fr{ d_xyz + (size_t)b0 * frame_stride, frame_stride, axis_stride, nb };
-        rc = enqueue_batch(p, *s, fr, frame_beg + b0, false);
-        release_slot(p, s);
-        if (rc) return rc;
+        rc = enqueue_batch(p, *s, fr, frame_beg + b0, SPACE_FULL); if (rc) return rc;
     }
     return 0;
 }
@@ -1376,13 +1379,13 @@ static int eval_host_frames_1(mdgpu_plan* p, const float* h_xyz, size_t frame_st
     int rc = ensure_slots(p, cell_at(cells, cell_stride_bytes, 0), true); if (rc) return rc;
     cudaPointerAttributes attr{}; bool pinned = false;
     if (cudaPointerGetAttributes(&attr, h_xyz) == cudaSuccess) pinned = (attr.type == cudaMemoryTypeHost); else cudaGetLastError();
-    const bool c = p->compact;
-    const size_t N = p->num_atoms, AS = c ? p->axis_stride_c : p->axis_stride, M = p->num_atoms_c;
+    const Space sp = p->ingest_space(); const bool c = sp == SPACE_COMPACT;
+    const size_t N = p->num_atoms, AS = p->space[sp].axis_stride, M = p->space[SPACE_COMPACT].num_atoms;
     std::vector<cudaEvent_t> direct;   // copies that read the caller's buffer: it may be refilled once they are done
     for (uint32_t b0 = 0; b0 < count; b0 += p->B) {
         if (p->interrupt.load()) return fail(MDGPU_ERR_INTERRUPTED, "evaluation interrupted");
         const uint32_t nb = std::min(p->B, count - b0);
-        Slot* s = nullptr; rc = acquire_slot(p, &s); if (rc) return rc;
+        SlotLease s; rc = acquire_slot(p, s); if (rc) return rc;
         for (uint32_t i = 0; i < nb; ++i) s->h_cells[i] = *cell_at(cells, cell_stride_bytes, b0 + i);
         const float* src = h_xyz + (size_t)b0 * frame_stride;
         cudaError_t e = cudaSuccess;
@@ -1410,11 +1413,9 @@ static int eval_host_frames_1(mdgpu_plan* p, const float* h_xyz, size_t frame_st
                 memcpy(s->h_frames.get() + ((size_t)i * 3 + ax) * AS, src + (size_t)i * frame_stride + (size_t)ax * axis_stride, sizeof(float) * N);
             e = cudaMemcpyAsync(s->d_frames.get(), s->h_frames.get(), sizeof(float) * (size_t)nb * 3 * AS, cudaMemcpyHostToDevice, s->stream);
         }
-        if (e != cudaSuccess) { release_slot(p, s); return fail(MDGPU_ERR_CUDA, "H2D copy failed: %s", cudaGetErrorString(e)); }
+        if (e != cudaSuccess) return fail(MDGPU_ERR_CUDA, "H2D copy failed: %s", cudaGetErrorString(e));
         BatchFrames fr{ s->d_frames.get(), 3 * AS, AS, nb };
-        rc = enqueue_batch(p, *s, fr, frame_beg + b0, c);
-        release_slot(p, s);
-        if (rc) return rc;
+        rc = enqueue_batch(p, *s, fr, frame_beg + b0, sp); if (rc) return rc;
     }
     // "copied host->device batch by batch inside the call": when the call returns, the caller's buffer has been read
     for (cudaEvent_t ev : direct) CUDA_TRY(cudaEventSynchronize(ev));
@@ -1472,7 +1473,7 @@ int mdgpu_eval_xtc_frames(mdgpu_plan* p, const uint8_t* h_blob, const uint64_t* 
     if (p->multi) return fail(MDGPU_ERR_UNSUPPORTED, "XTC input is evaluated on one device; create a single-device plan");
     std::lock_guard<std::mutex> xtc_guard(p->xtc_mutex);   // the scan stages are one pipeline: one XTC evaluation at a time per plan
     int rc = ensure_slots(p, &first, false); if (rc) return rc;
-    const size_t AS = p->axis_stride, NA = p->num_atoms;
+    const size_t AS = p->space[SPACE_FULL].axis_stride, NA = p->num_atoms;
     const uint32_t SB = p->B * XTC_SUPER;
     const uint32_t nsuper = (count + SB - 1) / SB;
     // stage k+1 (copy + scan, on its own stream) is issued BEFORE the batches of stage k are enqueued, so it overlaps their kernels
@@ -1500,25 +1501,23 @@ int mdgpu_eval_xtc_frames(mdgpu_plan* p, const uint8_t* h_blob, const uint64_t* 
         for (uint32_t b0 = 0; b0 < ns; b0 += p->B) {
             if (p->interrupt.load()) return fail(MDGPU_ERR_INTERRUPTED, "evaluation interrupted");
             const uint32_t nb = std::min(p->B, ns - b0);
-            Slot* sp = nullptr; rc = acquire_slot(p, &sp); if (rc) return rc;
-            Slot& s = *sp;
+            SlotLease lease; rc = acquire_slot(p, lease); if (rc) return rc;
+            Slot& s = *lease;
             bool ok = true;
             for (uint32_t i = 0; i < nb && ok; ++i) {
                 const uint64_t o = frame_offsets[s0 + b0 + i];
                 ok = xtc_header_cell(h_blob + o, (size_t)(frame_offsets[s0 + b0 + i + 1] - o), &s.h_cells[i], nullptr, nullptr);
             }
-            if (!ok) { release_slot(p, sp); return fail(MDGPU_ERR_FRAME_SOURCE, "XTC: Magic number did not match"); }
+            if (!ok) return fail(MDGPU_ERR_FRAME_SOURCE, "XTC: Magic number did not match");
             cudaError_t e = cudaSuccess;
             if (!s.d_xtc_frames.get()) e = s.d_xtc_frames.alloc((size_t)p->B * 3 * AS);   // whole decoded frames (global atom indices)
             if (e == cudaSuccess) e = cudaStreamWaitEvent(s.stream, st.ready, 0);
-            if (e != cudaSuccess) { release_slot(p, sp); return fail(MDGPU_ERR_CUDA, "XTC stage set-up failed: %s", cudaGetErrorString(e)); }
+            if (e != cudaSuccess) return fail(MDGPU_ERR_CUDA, "XTC stage set-up failed: %s", cudaGetErrorString(e));
             launch_xtc_expand(st.d_blob.get(), st.d_off.get() + b0, (uint32_t)NA, (int)nb, st.d_info.get() + b0, st.d_rec.get() + (size_t)b0 * NA, st.d_state.get() + (size_t)b0 * NA, NA,
                               s.d_xtc_frames.get(), 3 * AS, AS, s.d_err.get(), s.stream);
             cudaEventRecord(st.consumed[st.n_consumed++], s.stream);
             BatchFrames fr{ s.d_xtc_frames.get(), 3 * AS, AS, nb };
-            rc = enqueue_batch(p, s, fr, frame_beg + s0 + b0, false);
-            release_slot(p, sp);
-            if (rc) return rc;
+            rc = enqueue_batch(p, s, fr, frame_beg + s0 + b0, SPACE_FULL); if (rc) return rc;
         }
     }
     p->next_xtc += nsuper;
@@ -1623,31 +1622,33 @@ int mdgpu_eval_trajectory(mdgpu_plan* p, const mdgpu_trajectory_i* traj, uint32_
 static int eval_trajectory_1(mdgpu_plan* p, const mdgpu_trajectory_i* traj, uint32_t frame_beg, uint32_t frame_end, uint32_t loader_threads) {
     CUDA_TRY(cudaSetDevice(p->device));
     const uint32_t T = std::max(1u, std::min(loader_threads ? loader_threads : 4u, 64u));
-    std::vector<mdgpu_trajectory_reader_i> readers(T);
-    for (uint32_t t = 0; t < T; ++t) { memset(&readers[t], 0, sizeof(readers[t])); if (!traj->init_reader(&readers[t], traj->inst)) return fail(MDGPU_ERR_FRAME_SOURCE, "Failed to initialize trajectory reader for evaluation"); }
-    auto free_readers = [&]() { for (auto& r : readers) if (r.free) r.free(&r); };
-    const bool c = p->compact;
-    const size_t ASF = p->axis_stride, AS = c ? p->axis_stride_c : p->axis_stride, M = p->num_atoms_c;
+    struct Readers { std::vector<mdgpu_trajectory_reader_i> v; ~Readers() { for (auto& r : v) if (r.free) r.free(&r); } } owner;   // this call's readers, freed when it returns
+    std::vector<mdgpu_trajectory_reader_i>& readers = owner.v; readers.resize(T);
+    memset(readers.data(), 0, sizeof(readers[0]) * T);
+    for (uint32_t t = 0; t < T; ++t) if (!traj->init_reader(&readers[t], traj->inst)) return fail(MDGPU_ERR_FRAME_SOURCE, "Failed to initialize trajectory reader for evaluation");
+    const Space sp = p->ingest_space(); const bool c = sp == SPACE_COMPACT;
+    const size_t ASF = p->space[SPACE_FULL].axis_stride, AS = p->space[sp].axis_stride, M = p->space[SPACE_COMPACT].num_atoms;
     {   // initial configuration = frame 0 (md_script.c:5808); the first caller loads it
         std::lock_guard<std::mutex> guard(p->init_mutex);
         if (!p->have_init) {
             std::vector<float> tmp(3 * ASF); mdgpu_frame_header_t fh{};
-            if (!readers[0].load_frame(readers[0].inst, 0, &fh, tmp.data(), tmp.data() + ASF, tmp.data() + 2 * ASF)) { free_readers(); return fail(MDGPU_ERR_FRAME_SOURCE, "Failed to load frame during evaluation"); }
-            int rc = mdgpu_plan_set_initial_frame(p, tmp.data(), tmp.data() + ASF, tmp.data() + 2 * ASF, &fh.unitcell); if (rc) { free_readers(); return rc; }
+            if (!readers[0].load_frame(readers[0].inst, 0, &fh, tmp.data(), tmp.data() + ASF, tmp.data() + 2 * ASF)) return fail(MDGPU_ERR_FRAME_SOURCE, "Failed to load frame during evaluation");
+            int rc = mdgpu_plan_set_initial_frame(p, tmp.data(), tmp.data() + ASF, tmp.data() + 2 * ASF, &fh.unitcell); if (rc) return rc;
         }
     }
     std::vector<std::vector<float>> scratch(c ? T : 0);
     for (auto& v : scratch) v.resize(3 * ASF);
-    int rc = 0; bool slots_ready = false;
-    for (uint32_t b0 = frame_beg; b0 < frame_end && !rc; b0 += p->B) {
-        if (p->interrupt.load()) { rc = fail(MDGPU_ERR_INTERRUPTED, "evaluation interrupted"); break; }
+    bool slots_ready = false;
+    for (uint32_t b0 = frame_beg; b0 < frame_end; b0 += p->B) {
+        if (p->interrupt.load()) return fail(MDGPU_ERR_INTERRUPTED, "evaluation interrupted");
         const uint32_t nb = std::min(p->B, frame_end - b0);
         if (!slots_ready) {   // need one header for the cell capacity
             mdgpu_frame_header_t fh{}; if (!readers[0].load_frame(readers[0].inst, b0, &fh, nullptr, nullptr, nullptr)) fh.unitcell = p->init_cell;
-            rc = ensure_slots(p, &fh.unitcell, true); if (rc) break; slots_ready = true;
+            const int rc = ensure_slots(p, &fh.unitcell, true); if (rc) return rc;
+            slots_ready = true;
         }
-        Slot* sp = nullptr; rc = acquire_slot(p, &sp); if (rc) break;
-        Slot& s = *sp;
+        SlotLease lease; int rc = acquire_slot(p, lease); if (rc) return rc;
+        Slot& s = *lease;
         std::atomic<int> failed{0};
         auto work = [&](uint32_t t) {
             for (uint32_t i = t; i < nb; i += T) {
@@ -1663,15 +1664,13 @@ static int eval_trajectory_1(mdgpu_plan* p, const mdgpu_trajectory_i* traj, uint
         };
         if (T == 1) work(0);
         else { std::vector<std::thread> th; for (uint32_t t = 0; t < T; ++t) th.emplace_back(work, t); for (auto& x : th) x.join(); }
-        if (failed) { release_slot(p, sp); rc = fail(MDGPU_ERR_FRAME_SOURCE, "Failed to load frame during evaluation"); break; }
+        if (failed) return fail(MDGPU_ERR_FRAME_SOURCE, "Failed to load frame during evaluation");
         cudaError_t e = cudaMemcpyAsync(s.d_frames.get(), s.h_frames.get(), sizeof(float) * (size_t)nb * 3 * AS, cudaMemcpyHostToDevice, s.stream);
-        if (e != cudaSuccess) { release_slot(p, sp); rc = fail(MDGPU_ERR_CUDA, "H2D copy failed: %s", cudaGetErrorString(e)); break; }
+        if (e != cudaSuccess) return fail(MDGPU_ERR_CUDA, "H2D copy failed: %s", cudaGetErrorString(e));
         BatchFrames fr{ s.d_frames.get(), 3 * AS, AS, nb };
-        rc = enqueue_batch(p, s, fr, b0, c);
-        release_slot(p, sp);
+        rc = enqueue_batch(p, s, fr, b0, sp); if (rc) return rc;
     }
-    free_readers();
-    return rc;
+    return 0;
 }
 
 extern "C" {
@@ -1696,26 +1695,33 @@ static void temporal_ranges(Prop& pr) {
 
 // Fold the device accumulators of the distribution / volume properties into the host-visible property data, over the frames in `done`.
 // `st`: stream the copies run on (the fold of a running evaluation uses the plan's publication stream and never drains the device).
+// A distribution's accumulator -> acc[1024], and its per-frame minimum / maximum rows reduced over the frames in `done` into the property's
+// min_value / max_value; `value` turns a row entry into the reported float. Waits for `st` (and so for copies the caller enqueued before).
+template <typename T, typename V> static int fold_distribution(Prop& pr, const DevBuf<T>& d_min, const DevBuf<T>& d_max, const std::vector<uint32_t>& done, std::vector<unsigned long long>& acc, V&& value, cudaStream_t st) {
+    std::vector<T> mn(d_min.size()), mx(d_max.size()); acc.resize(MDGPU_DIST_BINS);
+    CUDA_TRY(cudaMemcpyAsync(acc.data(), pr.d_acc.get(), sizeof(unsigned long long) * MDGPU_DIST_BINS, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(mn.data(), d_min.get(), d_min.bytes(), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(mx.data(), d_max.get(), d_max.bytes(), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    float vmin = +FLT_MAX, vmax = -FLT_MAX;
+    for (uint32_t f : done) { vmin = std::min(vmin, value(mn[f])); vmax = std::max(vmax, value(mx[f])); }
+    pr.data.min_value = vmin; pr.data.max_value = vmax;
+    return 0;
+}
+
 static int fold_accumulators(mdgpu_plan* p, const std::vector<uint32_t>& done, uint64_t evaluated, cudaStream_t st) {
-    const size_t F = p->num_frames;
     for (auto& pr : p->props) {
         // mean divisor = number of frame evaluations that went into the accumulators (the reference's count++ moving average, md_script.c:5912:
         // a frame evaluated twice counts twice); after a cross-GPU exchange the caller states the global count
         const uint64_t n = pr.frames_overridden ? pr.frames_accumulated : evaluated;
         pr.data.frames_accumulated = n;
         if (pr.op == MDGPU_OP_RDF) {
-            std::vector<unsigned long long> acc(MDGPU_DIST_BINS), tot(F); std::vector<uint32_t> mn(F), mx(F);
-            CUDA_TRY(cudaMemcpyAsync(acc.data(), pr.d_acc.get(), sizeof(unsigned long long) * MDGPU_DIST_BINS, cudaMemcpyDeviceToHost, st));
-            CUDA_TRY(cudaMemcpyAsync(tot.data(), pr.d_frame_total.get(), sizeof(unsigned long long) * F, cudaMemcpyDeviceToHost, st));
-            CUDA_TRY(cudaMemcpyAsync(mn.data(), pr.d_frame_min.get(), sizeof(uint32_t) * F, cudaMemcpyDeviceToHost, st));
-            CUDA_TRY(cudaMemcpyAsync(mx.data(), pr.d_frame_max.get(), sizeof(uint32_t) * F, cudaMemcpyDeviceToHost, st));
-            CUDA_TRY(cudaStreamSynchronize(st));
+            std::vector<unsigned long long> acc, tot(p->num_frames);
+            CUDA_TRY(cudaMemcpyAsync(tot.data(), pr.d_frame_total.get(), pr.d_frame_total.bytes(), cudaMemcpyDeviceToHost, st));
+            { const int rc = fold_distribution(pr, pr.d_frame_min, pr.d_frame_max, done, acc, [](uint32_t v) { return (float)v; }, st); if (rc) return rc; }
             // mean of the per-frame integer bins: exact sum, one division (the reference keeps a float cumulative moving
             // average, md_script.c:5912-5921, which drifts by ~1e-5 from this value after 4096 frames: tests/test_oracle_golden.py)
             for (int b = 0; b < MDGPU_DIST_BINS; ++b) pr.vptr[b] = n ? (float)((double)acc[b] / (double)n) : 0.0f;
-            float vmin = +FLT_MAX, vmax = -FLT_MAX;
-            for (uint32_t f : done) { vmin = std::min(vmin, (float)mn[f]); vmax = std::max(vmax, (float)mx[f]); }
-            pr.data.min_value = vmin; pr.data.max_value = vmax;
             // weights of the last evaluated frame (the reference copies "whichever frame finished last", :5924); compute_rdf :5323-5337
             if (!done.empty()) {
                 const float min_cutoff = pr.cutoff_min > 1e-3f ? pr.cutoff_min : 1e-3f, max_cutoff = pr.cutoff_max;
@@ -1731,26 +1737,23 @@ static int fold_accumulators(mdgpu_plan* p, const std::vector<uint32_t>& done, u
             CUDA_TRY(cudaMemcpyAsync(pr.vptr, pr.d_vol_mean.get(), sizeof(float) * pr.values.size(), cudaMemcpyDeviceToHost, st));
             CUDA_TRY(cudaStreamSynchronize(st));
             // min_value / max_value are never updated for volumes in the reference (md_script.c:5936-5956)
-        } else if (pr.op >= MDGPU_OP_DENSITY_X && pr.op <= MDGPU_OP_DENSITY_Z) {
-            std::vector<unsigned long long> acc(MDGPU_DIST_BINS), mn(F), mx(F);
-            CUDA_TRY(cudaMemcpyAsync(acc.data(), pr.d_acc.get(), sizeof(unsigned long long) * MDGPU_DIST_BINS, cudaMemcpyDeviceToHost, st));
-            CUDA_TRY(cudaMemcpyAsync(mn.data(), pr.d_frame_min64.get(), sizeof(unsigned long long) * F, cudaMemcpyDeviceToHost, st));
-            CUDA_TRY(cudaMemcpyAsync(mx.data(), pr.d_frame_max64.get(), sizeof(unsigned long long) * F, cudaMemcpyDeviceToHost, st));
-            CUDA_TRY(cudaStreamSynchronize(st));
+        } else if (pr.is_density()) {
+            std::vector<unsigned long long> acc;
             const double unit = 1.0 / 16777216.0;
+            { const int rc = fold_distribution(pr, pr.d_frame_min64, pr.d_frame_max64, done, acc, [&](unsigned long long v) { return (float)((double)(float)((double)v * unit) * pr.dens_factor); }, st); if (rc) return rc; }
             for (int b = 0; b < MDGPU_DIST_BINS; ++b) pr.vptr[b] = n ? (float)(((double)acc[b] * unit / (double)n) * pr.dens_factor) : 0.0f;
             for (int b = 0; b < MDGPU_DIST_BINS; ++b) pr.vptr[MDGPU_DIST_BINS + b] = 1.0f;
-            float vmin = +FLT_MAX, vmax = -FLT_MAX;
-            for (uint32_t f : done) {
-                vmin = std::min(vmin, (float)((double)(float)((double)mn[f] * unit) * pr.dens_factor));
-                vmax = std::max(vmax, (float)((double)(float)((double)mx[f] * unit) * pr.dens_factor));
-            }
-            pr.data.min_value = vmin; pr.data.max_value = vmax;
             const float rad = pr.re * 0.5f;   // value_range {-rad, rad} (:4983-4995)
             pr.data.min_range[0] = -rad; pr.data.max_range[0] = rad;
         }
     }
     return 0;
+}
+
+// the frame mask as it stands now -> d_mask
+static cudaError_t upload_frame_mask(mdgpu_plan* p, DevBuf<unsigned long long>& d_mask) {
+    std::vector<uint64_t> mask; { std::lock_guard<std::mutex> lk(p->mask_mutex); mask = p->frame_mask; }
+    return d_mask.upload((const unsigned long long*)mask.data(), mask.size());
 }
 
 static void done_frames(mdgpu_plan* p, std::vector<uint32_t>& done) {
@@ -1843,10 +1846,8 @@ int mdgpu_plan_property_histogram(mdgpu_plan* p, size_t prop, uint32_t num_bins,
     Prop& pr = p->props[prop];
     if (!pr.d_temporal.get()) return fail(MDGPU_ERR_INVALID_ARG, "property '%s' is not a temporal", pr.name.c_str());
     const uint32_t dim = (uint32_t)pr.len, rows = aggregate ? 1u : dim;
-    std::vector<uint64_t> mask; { std::lock_guard<std::mutex> lk(p->mask_mutex); mask = p->frame_mask; }
     DevBuf<unsigned long long> d_mask; DevBuf<uint32_t> d_counts, d_tot;
-    if (d_mask.alloc(mask.size()) != cudaSuccess || d_counts.alloc((size_t)rows * num_bins) != cudaSuccess || d_tot.alloc(rows) != cudaSuccess) return fail(MDGPU_ERR_CUDA, "device allocation failed (histogram)");
-    cudaMemcpy(d_mask.get(), mask.data(), sizeof(uint64_t) * mask.size(), cudaMemcpyHostToDevice);
+    if (upload_frame_mask(p, d_mask) != cudaSuccess || d_counts.alloc((size_t)rows * num_bins) != cudaSuccess || d_tot.alloc(rows) != cudaSuccess) return fail(MDGPU_ERR_CUDA, "device allocation failed (histogram)");
     cudaMemset(d_counts.get(), 0, d_counts.bytes()); cudaMemset(d_tot.get(), 0, d_tot.bytes());
     const float range_ext = range_max - range_min, inv_range = range_ext > 0.0f ? 1.0f / range_ext : 0.0f;   // src/main.cpp:188-189
     launch_temporal_histogram(pr.d_temporal.get(), d_mask.get(), (uint32_t)p->num_frames, dim, range_min, range_max, inv_range, num_bins, aggregate, d_counts.get(), d_tot.get(), 0);
@@ -1888,14 +1889,13 @@ int mdgpu_plan_rama_density(mdgpu_plan* p, size_t prop, const uint32_t* segments
     if (!(sigma >= 0.1f && sigma <= 10.0f)) return fail(MDGPU_ERR_INVALID_ARG, "mdgpu_plan_rama_density: sigma %g outside [0.1, 10]", (double)sigma);
     int rc = mdgpu_plan_sync(p); if (rc) return rc;   // multi-device plans hold every frame's rows on devices[0] = p->device from here on
     CUDA_TRY(cudaSetDevice(p->device));
-    std::vector<uint64_t> mask; { std::lock_guard<std::mutex> lk(p->mask_mutex); mask = p->frame_mask; }
     const size_t texels = 512 * 512 * 4;
     RamaArgs a{};
     DevBuf<unsigned long long> d_mask, d_counts, d_samples; DevBuf<uint32_t> d_seg; DevBuf<float> d_buf;
-    if (d_mask.alloc(mask.size()) != cudaSuccess || d_seg.upload(segments ? segments + class_offsets[0] : nullptr, n_entries) != cudaSuccess ||
+    if (upload_frame_mask(p, d_mask) != cudaSuccess) return fail(MDGPU_ERR_CUDA, d_mask.get() ? "frame mask upload failed (rama density)" : "device allocation failed (rama density)");
+    if (d_seg.upload(segments ? segments + class_offsets[0] : nullptr, n_entries) != cudaSuccess ||
         d_counts.alloc(texels) != cudaSuccess || d_samples.alloc(4) != cudaSuccess || d_buf.alloc(3 * texels) != cudaSuccess)
         return fail(MDGPU_ERR_CUDA, "device allocation failed (rama density)");
-    if (cudaMemcpy(d_mask.get(), mask.data(), sizeof(uint64_t) * mask.size(), cudaMemcpyHostToDevice) != cudaSuccess) return fail(MDGPU_ERR_CUDA, "frame mask upload failed (rama density)");
     a.angles = pr.d_temporal.get(); a.n_seg = (uint32_t)pr.backbone_segments; a.seg = d_seg.get(); a.n_entries = n_entries;
     for (int c = 0; c < 3; ++c) a.class_end[c] = class_offsets[c + 1] - class_offsets[0];
     a.frame_beg = frame_beg; a.frame_count = frame_end - frame_beg; a.mask = d_mask.get();
@@ -1958,7 +1958,7 @@ int mdgpu_plan_bind_property_storage(mdgpu_plan* p, size_t prop, float* values, 
     { int rc = mdgpu_plan_sync(p); if (rc) return rc; }
     std::lock_guard<std::mutex> guard(p->sync_mutex);
     memcpy(values, pr.vptr, sizeof(float) * num_values);
-    pr.vptr = values; pr.bound = true; pr.data.values = values; pr.data.weights = pr.is_dist() ? values + MDGPU_DIST_BINS : nullptr;
+    pr.vptr = values; pr.data.values = values; pr.data.weights = pr.is_dist() ? values + MDGPU_DIST_BINS : nullptr;
     if (!pr.agg_mean.empty() && agg_mean && agg_var && agg_ext) {
         memcpy(agg_mean, pr.amean, sizeof(float) * p->num_frames); memcpy(agg_var, pr.avar, sizeof(float) * p->num_frames); memcpy(agg_ext, pr.aext, sizeof(float) * 2 * p->num_frames);
         pr.amean = agg_mean; pr.avar = agg_var; pr.aext = agg_ext;
@@ -2000,7 +2000,7 @@ int mdgpu_plan_exchange_stats(mdgpu_plan* p, double* last_ms, uint64_t* count) {
 }
 int mdgpu_plan_ingest_info(mdgpu_plan* p, size_t* atoms_per_frame, uint32_t* threads) {
     if (!p) return fail(MDGPU_ERR_INVALID_ARG, "null plan");
-    if (atoms_per_frame) *atoms_per_frame = p->compact ? p->num_atoms_c : p->num_atoms;
+    if (atoms_per_frame) *atoms_per_frame = p->space[p->ingest_space()].num_atoms;
     if (threads) *threads = p->compact ? (uint32_t)(ingest_pool(p)->th.size() + 1) : 0u;
     return 0;
 }
@@ -2044,7 +2044,7 @@ int mdgpu_plan_property_frame_rows(mdgpu_plan* p, size_t prop, uint32_t which, v
 
 int mdgpu_plan_mark_frames_done(mdgpu_plan* p, uint32_t frame_beg, uint32_t count) {
     if (!p || (size_t)frame_beg + count > p->num_frames) return fail(MDGPU_ERR_INVALID_ARG, "mdgpu_plan_mark_frames_done: frame range out of bounds");
-    { std::lock_guard<std::mutex> lk(p->mask_mutex); for (uint32_t f = frame_beg; f < frame_beg + count; ++f) p->frame_mask[f >> 6] |= 1ull << (f & 63); }
+    mark_frames(p, frame_beg, count);
     p->dirty = true;
     return 0;
 }
@@ -2159,18 +2159,24 @@ int mdgpu_synth_water_frames_host(uint32_t n, uint32_t seed, const float* base_x
     return 0;
 }
 
-int mdgpu_synth_water_frames_device(int device, uint32_t n, uint32_t seed, const float* d_base_xyz, uint32_t frame_beg, uint32_t count,
-                                    float* d_out_xyz, size_t frame_stride, size_t axis_stride) {
-    if (!d_base_xyz || !d_out_xyz) return fail(MDGPU_ERR_INVALID_ARG, "null argument");
+// frames [frame_beg, frame_beg + count) of a synthetic trajectory, 32768 frames per launch (mol_id null: water)
+static int synth_frames_device(int device, uint32_t seed, float Lx, float Ly, float Lz, uint32_t num_atoms, const float* d_base_xyz, const uint32_t* d_mol_id,
+                               uint32_t frame_beg, uint32_t count, float* d_out_xyz, size_t frame_stride, size_t axis_stride) {
     CUDA_TRY(cudaSetDevice(device));
-    const mdsynth_water_t w = mdsynth_water_desc(n, seed);
     for (uint32_t c0 = 0; c0 < count; c0 += 32768) {
         const uint32_t c = std::min(32768u, count - c0);
-        launch_synth_frames(seed, w.L, w.L, w.L, w.num_atoms, d_base_xyz, w.num_atoms, nullptr, frame_beg + c0, c, d_out_xyz + (size_t)c0 * frame_stride, frame_stride, axis_stride, 0);
+        launch_synth_frames(seed, Lx, Ly, Lz, num_atoms, d_base_xyz, num_atoms, d_mol_id, frame_beg + c0, c, d_out_xyz + (size_t)c0 * frame_stride, frame_stride, axis_stride, 0);
     }
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaDeviceSynchronize());
     return 0;
+}
+
+int mdgpu_synth_water_frames_device(int device, uint32_t n, uint32_t seed, const float* d_base_xyz, uint32_t frame_beg, uint32_t count,
+                                    float* d_out_xyz, size_t frame_stride, size_t axis_stride) {
+    if (!d_base_xyz || !d_out_xyz) return fail(MDGPU_ERR_INVALID_ARG, "null argument");
+    const mdsynth_water_t w = mdsynth_water_desc(n, seed);
+    return synth_frames_device(device, seed, w.L, w.L, w.L, w.num_atoms, d_base_xyz, nullptr, frame_beg, count, d_out_xyz, frame_stride, axis_stride);
 }
 
 int mdgpu_synth_membrane_desc(uint32_t nl, uint32_t nw_xy, uint32_t nwz, uint32_t seed, uint32_t* num_atoms, uint32_t* num_lipids, float* L3) {
@@ -2200,15 +2206,8 @@ int mdgpu_synth_membrane_frames_host(uint32_t nl, uint32_t nw_xy, uint32_t nwz, 
 int mdgpu_synth_membrane_frames_device(int device, uint32_t nl, uint32_t nw_xy, uint32_t nwz, uint32_t seed, const float* d_base_xyz, const uint32_t* d_mol_id,
                                        uint32_t frame_beg, uint32_t count, float* d_out_xyz, size_t frame_stride, size_t axis_stride) {
     if (!d_base_xyz || !d_mol_id || !d_out_xyz) return fail(MDGPU_ERR_INVALID_ARG, "null argument");
-    CUDA_TRY(cudaSetDevice(device));
     const mdsynth_membrane_t m = mdsynth_membrane_desc(nl, nw_xy, nwz, seed);
-    for (uint32_t c0 = 0; c0 < count; c0 += 32768) {
-        const uint32_t c = std::min(32768u, count - c0);
-        launch_synth_frames(seed, m.Lx, m.Ly, m.Lz, m.num_atoms, d_base_xyz, m.num_atoms, d_mol_id, frame_beg + c0, c, d_out_xyz + (size_t)c0 * frame_stride, frame_stride, axis_stride, 0);
-    }
-    CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaDeviceSynchronize());
-    return 0;
+    return synth_frames_device(device, seed, m.Lx, m.Ly, m.Lz, m.num_atoms, d_base_xyz, d_mol_id, frame_beg, count, d_out_xyz, frame_stride, axis_stride);
 }
 
 // ------------------------------------------------------------------------------------------------- memory helpers
