@@ -140,6 +140,8 @@ typedef enum mdgpu_op {
  *              `selection and within(...)` (_and :1975) and idx[2] holds that static selection's atoms (possibly none).
  *   WITHIN_COUNT: idx[0] = the selection's atoms, cutoff_max = radius (> 0), cutoff_min = lower bound of the min:max form (else 0). The dynamic selection within() is evaluated per frame over the
  *              system-wide cell list (get_spatial_acc :734); so far its only consumer on the device is count().
+ *              count(<coordinate range> [and static]): a mdgpu_range_arg_t for argument 0, its static side in dyn[0], idx[0] empty and
+ *              cutoff_min = cutoff_max = 0; the count of the frame's selected atoms (_count :2868).
  *   SHAPE_WEIGHTS: idx[0] = the atoms of num_structures structures back to back (structure_offsets, or structure_size each), bit 0 of com_args
  *              = weights are the atom masses (shapespace's use_mass; _shape_weights always uses them), else 1.
  *   COORD_X/_Y/_Z: idx[0] = the atoms.
@@ -173,7 +175,9 @@ typedef enum mdgpu_op {
  *              trigonometric centre of mass _com_pbc_iw :7850, 8-lane float accumulation as in the AVX2 build). */
 /* A dynamic selection as an argument: within([radius_min:]radius_max, selection) [and static_selection] (_within_expl_flt / _frng
  * md_script_functions.inl:2485-2720, `and` :1975), evaluated per frame on the device over the system-wide cell list (get_spatial_acc :734).
- * For argument k of a property, idx[k] holds the atoms of the within() selection and dyn[k] the rest. */
+ * For argument k of a property, idx[k] holds the atoms of the within() selection and dyn[k] the rest.
+ *
+ * An argument can instead be a coordinate range: see mdgpu_range_arg_t below. */
 typedef struct mdgpu_dynamic_arg_t {
     float radius_min, radius_max;   /* radius_max > 0 switches the argument to dynamic */
     const int32_t* and_idx;         /* the static side of `selection and within(...)`, or NULL */
@@ -243,6 +247,29 @@ int mdgpu_device_count(void);
 /* Plan lifetime. num_frames is the trajectory length (rows of temporal properties; md_script_eval_create :6506). */
 mdgpu_plan* mdgpu_plan_create(const mdgpu_system_desc_t* sys, const mdgpu_property_desc_t* props, size_t num_props,
                               size_t num_frames, const mdgpu_plan_options_t* opts);
+
+/* A coordinate range as argument `arg` of property `prop`: within_x(a:b) / within_y(a:b) / within_z(a:b) / within_xyz(a:b, c:d, e:f)
+ * [and static_selection] (procedures md_script_functions.inl:668-671, coordinate_range :2394-2476), evaluated per frame on the device.
+ * Atom i of the frame is selected iff lo[0] <= x[i] <= hi[0] and the same for y and z: the frame's coordinates as loaded (no wrapping, no cell,
+ * orthorhombic or triclinic: atoms of unwrapped trajectories outside the cell count by their raw coordinates), both ends inclusive. An axis the
+ * call does not constrain is [-FLT_MAX, FLT_MAX]; it is still compared, so an atom with a NaN or +-inf coordinate on any axis is never selected.
+ * Integer bounds arrive as the frange the front end casts them to. Unlike within(), no atom is removed afterwards; `selection and within_*(...)`
+ * is the intersection: the static side is dyn[arg].and_idx / and_count / has_and of the property, whose radius_* stay 0; idx[arg] stays empty.
+ * A range is evaluated over all atoms of the system (:2414-2424); the form inside an `in` context (:2401-2412, only the context's atoms) is not
+ * lowered. Consumers: those of within() (see mdgpu_property_desc_t.dyn); count(<range expression>) is MDGPU_OP_WITHIN_COUNT with the range as
+ * argument 0 (cutoff_min = cutoff_max = 0).
+ * The ranges travel beside the property descriptors, not in them, so that the layout of mdgpu_property_desc_t stays that of hosts compiled
+ * before ranges existed. */
+typedef struct mdgpu_range_arg_t {
+    uint32_t prop;                  /* index into props */
+    uint32_t arg;                   /* argument 0..3 of that property */
+    float lo[3], hi[3];             /* x, y, z bounds, inclusive */
+} mdgpu_range_arg_t;
+/* mdgpu_plan_create with coordinate-range arguments. Fails with MDGPU_ERR_INVALID_ARG for a range whose prop / arg is out of range or listed twice,
+ * an argument with both a radius and a range, and a range with lo > hi or a NaN bound; with MDGPU_ERR_UNSUPPORTED where the procedure takes no
+ * dynamic selection. mdgpu_plan_create(...) is this function with no ranges. */
+mdgpu_plan* mdgpu_plan_create_with_ranges(const mdgpu_system_desc_t* sys, const mdgpu_property_desc_t* props, size_t num_props,
+                                          size_t num_frames, const mdgpu_plan_options_t* opts, const mdgpu_range_arg_t* ranges, size_t num_ranges);
 void mdgpu_plan_destroy(mdgpu_plan* plan);
 
 /* Frame 0 of the trajectory ("initial configuration", md_script.c:5808): reference structure of sdf() and rmsd(), reference cell of density_*(). */

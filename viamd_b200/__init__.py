@@ -4,8 +4,8 @@ The product is viamd_b200/libmdgpu.so (hand-written CUDA for sm_90a behind the C
 the thin host-side mirror of the md_script evaluation API used by the tests and bench.py.
 """
 from .api import (  # noqa: F401
-    MdgpuError, UnitCell, System, Property, PropertyData, Plan, Within, Trajectory, ArrayTrajectory,
-    rdf, rdf_com, rdf_within, sdf, density, distance, distance_min, distance_max, distance_pair, rmsd, porosity, com, plane, count_within, in_contexts, shape_weights, coord, angle, dihedral, backbone_angles, contact_count, water_system, device_count, bind_host_to_device, launch_count, lib,
+    MdgpuError, UnitCell, System, Property, PropertyData, Plan, Within, Range, Trajectory, ArrayTrajectory,
+    rdf, rdf_com, rdf_within, sdf, density, distance, distance_min, distance_max, distance_pair, rmsd, porosity, com, plane, count_within, count_range, in_contexts, shape_weights, coord, angle, dihedral, backbone_angles, contact_count, water_system, device_count, bind_host_to_device, launch_count, lib,
     synth_membrane_desc, synth_membrane_base, synth_membrane_frames_host, synth_membrane_frames_device, membrane_system,
     synth_water_desc, synth_water_base, synth_water_frames_host, synth_water_frames_device,
     xtc_frame_offsets, xtc_decode_frames,

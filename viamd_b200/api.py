@@ -71,6 +71,10 @@ class _DynArg(C.Structure):   # mdgpu_dynamic_arg_t
     _fields_ = [("radius_min", C.c_float), ("radius_max", C.c_float), ("and_idx", C.POINTER(C.c_int32)), ("and_count", C.c_size_t), ("has_and", C.c_uint32)]
 
 
+class _RangeArg(C.Structure):   # mdgpu_range_arg_t
+    _fields_ = [("prop", C.c_uint32), ("arg", C.c_uint32), ("lo", C.c_float * 3), ("hi", C.c_float * 3)]
+
+
 class _PropertyDesc(C.Structure):
     _fields_ = [("name", C.c_char_p), ("op", C.c_uint32), ("idx", C.POINTER(C.c_int32) * 4), ("idx_count", C.c_size_t * 4),
                 ("num_structures", C.c_size_t), ("structure_size", C.c_size_t), ("cutoff_min", C.c_float), ("cutoff_max", C.c_float),
@@ -129,6 +133,9 @@ def lib() -> C.CDLL:
         L.mdgpu_last_error.restype = C.c_char_p
         L.mdgpu_plan_create.restype = C.c_void_p
         L.mdgpu_plan_create.argtypes = [C.POINTER(_SystemDesc), C.POINTER(_PropertyDesc), C.c_size_t, C.c_size_t, C.POINTER(_PlanOptions)]
+        L.mdgpu_plan_create_with_ranges.restype = C.c_void_p
+        L.mdgpu_plan_create_with_ranges.argtypes = [C.POINTER(_SystemDesc), C.POINTER(_PropertyDesc), C.c_size_t, C.c_size_t, C.POINTER(_PlanOptions),
+                                                    C.POINTER(_RangeArg), C.c_size_t]
         L.mdgpu_plan_destroy.argtypes = [C.c_void_p]
         L.mdgpu_plan_destroy.restype = None
         L.mdgpu_plan_clear.argtypes = [C.c_void_p]
@@ -227,6 +234,7 @@ class Property:
     structure_offsets_b: Optional[np.ndarray] = None  # distance_pair: CSR groups of argument 1 (argument 0 uses structure_offsets)
     dyn: dict = field(default_factory=dict)           # {k: (radius_min, radius_max, and_idx | None)}: argument k is within([min:]max, idx[k]) [and and_idx], per frame
     arg_offsets: dict = field(default_factory=dict)   # {k: CSR offsets}: argument k of distance / angle / dihedral / com is an ARRAY of selections (centre of their centres)
+    ranges: dict = field(default_factory=dict)        # {k: Range}: argument k is a coordinate range within_x / _y / _z / _xyz(...) [and static], per frame
 
 
 class Within:
@@ -238,11 +246,38 @@ class Within:
         self.sel = np.asarray(sel_idx, np.int32); self.and_idx = None if and_idx is None else np.asarray(and_idx, np.int32)
 
 
-def _split_dyn(args):
-    """[index array | Within, ...] -> (idx lists, dyn dict)"""
+FLT_MAX = float(np.finfo(np.float32).max)
+
+
+class Range:
+    """within_x(a:b) / within_y / within_z / within_xyz(a:b, c:d, e:f) [and a static selection] as a property argument (coordinate_range
+    md_script_functions.inl:2394): per frame the atoms with lo <= (x, y, z) <= hi on every axis, by their raw coordinates; unconstrained axes are
+    [-FLT_MAX, FLT_MAX]. and_idx: the static side of `selection and within_*(...)` (None: no static side). Evaluated per frame on the device."""
+
+    def __init__(self, lo, hi, and_idx=None):
+        self.lo = np.asarray(lo, np.float32).reshape(3); self.hi = np.asarray(hi, np.float32).reshape(3)
+        self.and_idx = None if and_idx is None else np.asarray(and_idx, np.int32)
+
+    @staticmethod
+    def axis(axis, lo, hi, and_idx=None):
+        """within_x / _y / _z (axis 0 / 1 / 2)"""
+        l = [-FLT_MAX] * 3; h = [FLT_MAX] * 3; l[axis] = lo; h[axis] = hi
+        return Range(l, h, and_idx)
+
+    def mask(self, x, y, z):
+        """the selection of one frame (numpy, the reference's comparison)"""
+        m = (self.lo[0] <= x) & (x <= self.hi[0]) & (self.lo[1] <= y) & (y <= self.hi[1]) & (self.lo[2] <= z) & (z <= self.hi[2])
+        if self.and_idx is not None:
+            keep = np.zeros(len(m), bool); keep[self.and_idx] = True; m &= keep
+        return m
+
+
+def _split_dyn(args, ranges=None):
+    """[index array | Within | Range, ...] -> (idx lists, dyn dict); the coordinate ranges go to `ranges` (their idx list stays empty)"""
     idx, dyn = [], {}
     for k, a in enumerate(args):
         if isinstance(a, Within): idx.append(a.sel); dyn[k] = (a.radius_min, a.radius, a.and_idx)
+        elif isinstance(a, Range): idx.append(np.zeros(0, np.int32)); ranges[k] = a
         else: idx.append(np.asarray(a, np.int32))
     return idx, dyn
 
@@ -261,8 +296,8 @@ def rdf(name, ref_idx, trg_idx, cutoff, cutoff_min=0.0):
     """ref_idx / trg_idx: atom index arrays, or Within(...) for a selection evaluated per frame; trg_idx may be a list of index arrays (an array of
     selections: their centres of mass are the targets)"""
     trg_idx, toff = _trg_groups(trg_idx)
-    idx, dyn = _split_dyn([ref_idx, trg_idx])
-    return Property(name, OP_RDF, idx, cutoff_min=float(cutoff_min), cutoff_max=float(cutoff), dyn=dyn, structure_offsets_b=toff)
+    rng = {}; idx, dyn = _split_dyn([ref_idx, trg_idx], rng)
+    return Property(name, OP_RDF, idx, cutoff_min=float(cutoff_min), cutoff_max=float(cutoff), dyn=dyn, structure_offsets_b=toff, ranges=rng)
 
 
 def rdf_within(name, radius, sel_idx, trg_idx, cutoff, cutoff_min=0.0, radius_min=0.0, and_idx=None):
@@ -286,13 +321,13 @@ def rdf_com(name, groups, trg_idx, cutoff, cutoff_min=0.0):
 def sdf(name, structures, trg_idx, cutoff):
     s = np.ascontiguousarray(structures, np.int32)
     assert s.ndim == 2, "structures: [num_structures, structure_size] atom indices"
-    idx, dyn = _split_dyn([s.reshape(-1), trg_idx])
-    return Property(name, OP_SDF, idx, num_structures=s.shape[0], structure_size=s.shape[1], cutoff_max=float(cutoff), dyn=dyn)
+    rng = {}; idx, dyn = _split_dyn([s.reshape(-1), trg_idx], rng)
+    return Property(name, OP_SDF, idx, num_structures=s.shape[0], structure_size=s.shape[1], cutoff_max=float(cutoff), dyn=dyn, ranges=rng)
 
 
 def density(name, axis, idx):
-    lst, dyn = _split_dyn([idx])
-    return Property(name, OP_DENSITY_X + int(axis), lst, dyn=dyn)
+    rng = {}; lst, dyn = _split_dyn([idx], rng)
+    return Property(name, OP_DENSITY_X + int(axis), lst, dyn=dyn, ranges=rng)
 
 
 def in_contexts(name, op, local_idx, context_first_atoms):
@@ -313,9 +348,10 @@ def in_contexts(name, op, local_idx, context_first_atoms):
 def _temporal(name, op, args):
     """each argument: an int (0-based atom index -> that atom's position) or an index array (a selection -> centre of mass,
     coordinate_extract_com md_script_functions.inl:1717)"""
-    idx, mask, dyn, parts = [], 0, {}, {}
+    idx, mask, dyn, parts, rng = [], 0, {}, {}, {}
     for k, a in enumerate(args):
         if isinstance(a, Within): idx.append(a.sel); mask |= 1 << k; dyn[k] = (a.radius_min, a.radius, a.and_idx)   # the frame's dynamic selection: its centre of mass
+        elif isinstance(a, Range): idx.append(np.zeros(0, np.int32)); mask |= 1 << k; rng[k] = a
         elif isinstance(a, list):   # an ARRAY of selections: the centre of the selections' centres (coordinate_extract_com :1826-1842)
             sels = [np.asarray(g, np.int32) for g in a]; mask |= 1 << k
             if len(sels) == 1: idx.append(sels[0])
@@ -324,7 +360,7 @@ def _temporal(name, op, args):
                 idx.append(np.concatenate(sels).astype(np.int32)); parts[k] = off
         elif np.ndim(a) == 0: idx.append(np.asarray([int(a)], np.int32))
         else: idx.append(np.asarray(a, np.int32)); mask |= 1 << k
-    return Property(name, op, idx, com_args=mask, dyn=dyn, arg_offsets=parts)
+    return Property(name, op, idx, com_args=mask, dyn=dyn, arg_offsets=parts, ranges=rng)
 
 
 def distance(name, a, b):
@@ -344,8 +380,8 @@ def _groups_or_idx(args):
 
 def _min_distance(name, op, a_idx, b_idx):
     (a_idx, b_idx), offs = _groups_or_idx([a_idx, b_idx])
-    idx, dyn = _split_dyn([a_idx, b_idx])
-    return Property(name, op, idx, dyn=dyn, num_structures=0 if offs[0] is None else len(offs[0]) - 1, structure_offsets=offs[0], structure_offsets_b=offs[1])
+    rng = {}; idx, dyn = _split_dyn([a_idx, b_idx], rng)
+    return Property(name, op, idx, dyn=dyn, num_structures=0 if offs[0] is None else len(offs[0]) - 1, structure_offsets=offs[0], structure_offsets_b=offs[1], ranges=rng)
 
 
 def distance_min(name, a_idx, b_idx):
@@ -388,6 +424,12 @@ def count_within(name, radius, sel_idx, radius_min=0.0, and_idx=None):
     selection itself excluded (_within_expl_flt md_script_functions.inl:2485, _count :2868) — a dynamic selection evaluated on the device"""
     idx = [np.asarray(sel_idx, np.int32)] + ([np.zeros(0, np.int32), np.asarray(and_idx, np.int32)] if and_idx is not None else [])
     return Property(name, OP_WITHIN_COUNT, idx, cutoff_min=float(radius_min), cutoff_max=float(radius), com_args=0 if and_idx is None else 1)   # min:max form: _within_expl_frng :2609
+
+
+def count_range(name, rng: Range):
+    """count(within_x / _y / _z / _xyz(...) [and static]): per frame the number of atoms in the coordinate range (coordinate_range
+    md_script_functions.inl:2394, _count :2868) — MDGPU_OP_WITHIN_COUNT with the range as dyn[0]"""
+    return Property(name, OP_WITHIN_COUNT, [np.zeros(0, np.int32)], ranges={0: rng})
 
 
 def shape_weights(name, groups, use_mass=True):
@@ -562,7 +604,7 @@ class Plan:
             rad = np.ascontiguousarray(system.radius, np.float32); self._keep.append(rad)
             if rad.shape != (system.num_atoms,): raise ValueError("System.radius: one radius per atom expected")
             sd.atom_radius = rad.ctypes.data_as(C.POINTER(C.c_float))
-        descs = (_PropertyDesc * len(self.properties))()
+        descs = (_PropertyDesc * len(self.properties))(); ranges = []
         for i, p in enumerate(self.properties):
             d = descs[i]; nm = p.name.encode(); self._keep.append(nm)
             d.name = nm; d.op = p.op; d.num_structures = p.num_structures; d.structure_size = p.structure_size
@@ -580,6 +622,11 @@ class Plan:
             for k, off in p.arg_offsets.items():
                 ao = np.ascontiguousarray(off, np.uint32); self._keep.append(ao)
                 d.arg_offsets[k] = ao.ctypes.data_as(C.POINTER(C.c_uint32)); d.arg_parts[k] = len(ao) - 1
+            for k, r in p.ranges.items():   # beside the descriptors: mdgpu_range_arg_t; the static side in dyn[k]
+                ranges.append((i, k, r))
+                if r.and_idx is not None:
+                    m = np.ascontiguousarray(r.and_idx, np.int32); self._keep.append(m)
+                    d.dyn[k].and_idx = m.ctypes.data_as(C.POINTER(C.c_int32)); d.dyn[k].and_count = m.size; d.dyn[k].has_and = 1
             for k, (rmin, rmax, and_idx) in p.dyn.items():
                 d.dyn[k].radius_min = rmin; d.dyn[k].radius_max = rmax
                 if and_idx is not None:
@@ -591,7 +638,14 @@ class Plan:
         if devices:
             o.num_devices = len(devices)
             for g, dv in enumerate(devices): o.devices[g] = int(dv)
-        self._h = L.mdgpu_plan_create(C.byref(sd), descs, len(self.properties), self.num_frames, C.byref(o))
+        if ranges:
+            rarr = (_RangeArg * len(ranges))()
+            for j, (i, k, r) in enumerate(ranges):
+                rarr[j].prop = i; rarr[j].arg = k
+                for c in range(3): rarr[j].lo[c] = float(r.lo[c]); rarr[j].hi[c] = float(r.hi[c])
+            self._h = L.mdgpu_plan_create_with_ranges(C.byref(sd), descs, len(self.properties), self.num_frames, C.byref(o), rarr, len(ranges))
+        else:
+            self._h = L.mdgpu_plan_create(C.byref(sd), descs, len(self.properties), self.num_frames, C.byref(o))
         if not self._h:
             raise MdgpuError(L.mdgpu_last_error().decode(errors="replace"))
         self._names = [p.name for p in self.properties]

@@ -116,6 +116,17 @@ struct WithinArgs {
 void launch_within_count(const WithinArgs& a, int B, bool tri, int sm_count, cudaStream_t s);
 // the same marks as a per-frame ascending index list (dyn_idx [B][num_atoms], dyn_n [B]); consumers take it as a DynSel
 void launch_within_list(const WithinArgs& a, int B, bool tri, int sm_count, int32_t* d_dyn_idx, uint32_t* d_dyn_n, cudaStream_t s);
+// within_x / _y / _z / _xyz(...) [and static] (coordinate_range md_script_functions.inl:2394): marks -> the same per-frame list / count
+struct RangeArgs {
+    BatchFrames frames;
+    float lo[3], hi[3];              // inclusive bounds per axis; unconstrained axes are [-FLT_MAX, FLT_MAX]
+    uint32_t has_and;                // 1: `selection and within_*(...)`: only the static side's atoms and_idx[0 .. n_and) are tested; 0: every atom
+    const int32_t* and_idx; uint32_t n_and;
+    uint32_t num_atoms;
+    uint8_t* flags;                  // [B][num_atoms]
+};
+void launch_range_list(const RangeArgs& a, int B, int sm_count, int32_t* d_dyn_idx, uint32_t* d_dyn_n, cudaStream_t s);
+void launch_range_count(const RangeArgs& a, int B, int sm_count, float* d_out, uint32_t frame0, cudaStream_t s);
 void launch_scan_home_cells(const FrameGeom* d_geom, const CellList& cl, int B, cudaStream_t s);   // cells.cu: k_scan_cells<1> alone
 
 // props.cu

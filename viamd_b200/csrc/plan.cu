@@ -20,6 +20,7 @@
 #include <thread>
 #include <type_traits>
 #include <utility>
+#include <array>
 #include <vector>
 #include <map>
 #include <memory>
@@ -116,8 +117,13 @@ struct Prop {
     std::vector<uint32_t> h_aoff[4]; DevBuf<uint32_t> d_aoff[4];   // distance / angle / dihedral / com: argument k is an ARRAY of selections (centre of their centres)
     DevBuf<uint8_t> d_and_mask;   // `selection and within(...)`: one byte per atom of the static side (count(within()) / rdf(within()))
     // Dynamic arguments: argument k is within([rmin:]rmax, h_idx[k]) [and a static selection], evaluated per frame on the device into an ascending
-    // index list (md_script_functions.inl:2485-2720); the consumers read that list instead of the static one.
-    struct DynArg { bool on = false; float rmin = 0.f, rmax = 0.f; DevBuf<uint8_t> d_and_mask; } dyn[4];
+    // index list (md_script_functions.inl:2485-2720); the consumers read that list instead of the static one. A coordinate range (`range`:
+    // within_x / _y / _z / _xyz, coordinate_range :2394) marks the atoms inside [lo, hi] instead, testing only the static side's atoms (d_and_idx)
+    // when it has one; count() of a range is dyn[0] of its MDGPU_OP_WITHIN_COUNT property.
+    struct DynArg {
+        bool on = false; float rmin = 0.f, rmax = 0.f; DevBuf<uint8_t> d_and_mask;
+        bool range = false; float lo[3] = {}, hi[3] = {}; DevBuf<int32_t> d_and_idx; bool has_and = false;
+    } dyn[4];
     bool any_dyn() const { return dyn[0].on || dyn[1].on || dyn[2].on || dyn[3].on; }
     // device accumulators (the result accumulators are listed once, in for_each_accumulator)
     DevBuf<unsigned long long> d_acc;             // rdf: 1024 bins; density: 1024 fixed-point sums
@@ -414,7 +420,20 @@ uint64_t mdgpu_launch_count(bool reset) { return reset ? g_launches.exchange(0) 
 
 mdgpu_plan* mdgpu_plan_create(const mdgpu_system_desc_t* sys, const mdgpu_property_desc_t* props, size_t num_props, size_t num_frames,
                               const mdgpu_plan_options_t* opts) {
-    if (!sys || !props || !num_props || !num_frames || !sys->num_atoms) { fail(MDGPU_ERR_INVALID_ARG, "mdgpu_plan_create: invalid arguments"); return nullptr; }
+    return mdgpu_plan_create_with_ranges(sys, props, num_props, num_frames, opts, nullptr, 0);
+}
+
+mdgpu_plan* mdgpu_plan_create_with_ranges(const mdgpu_system_desc_t* sys, const mdgpu_property_desc_t* props, size_t num_props, size_t num_frames,
+                                          const mdgpu_plan_options_t* opts, const mdgpu_range_arg_t* ranges, size_t num_ranges) {
+    if (!sys || !props || !num_props || !num_frames || !sys->num_atoms || (num_ranges && !ranges)) { fail(MDGPU_ERR_INVALID_ARG, "mdgpu_plan_create: invalid arguments"); return nullptr; }
+    // the coordinate range of each (property, argument), if any
+    std::vector<std::array<const mdgpu_range_arg_t*, 4>> range_of(num_props, std::array<const mdgpu_range_arg_t*, 4>{});
+    for (size_t r = 0; r < num_ranges; ++r) {
+        const mdgpu_range_arg_t& ra = ranges[r];
+        if (ra.prop >= num_props || ra.arg >= 4) { fail(MDGPU_ERR_INVALID_ARG, "coordinate range %zu: property %u / argument %u out of range", r, ra.prop, ra.arg); return nullptr; }
+        if (range_of[ra.prop][ra.arg]) { fail(MDGPU_ERR_INVALID_ARG, "coordinate range %zu: argument %u of property %u has two ranges", r, ra.arg, ra.prop); return nullptr; }
+        range_of[ra.prop][ra.arg] = &ra;
+    }
     mdgpu_plan_options_t o{}; if (opts) o = *opts;
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { fail(MDGPU_ERR_CUDA, "no CUDA device available (libmdgpu has no CPU fallback)"); return nullptr; }
@@ -426,12 +445,12 @@ mdgpu_plan* mdgpu_plan_create(const mdgpu_system_desc_t* sys, const mdgpu_proper
             if (!getenv("MDGPU_ALLOW_DUPLICATE_DEVICES")) for (uint32_t h = 0; h < g; ++h) if (o.devices[h] == o.devices[g]) { fail(MDGPU_ERR_INVALID_ARG, "device %d listed twice", o.devices[g]); return nullptr; }
         }
         mdgpu_plan_options_t one = o; one.num_devices = 0; one.device = o.devices[0];
-        mdgpu_plan* root = mdgpu_plan_create(sys, props, num_props, num_frames, &one);
+        mdgpu_plan* root = mdgpu_plan_create_with_ranges(sys, props, num_props, num_frames, &one, ranges, num_ranges);
         if (!root) return nullptr;
         root->multi = new MultiDevice(); root->multi->devices.assign(o.devices, o.devices + o.num_devices);
         for (uint32_t g = 1; g < o.num_devices; ++g) {
             one.device = o.devices[g];
-            mdgpu_plan* q = mdgpu_plan_create(sys, props, num_props, num_frames, &one);
+            mdgpu_plan* q = mdgpu_plan_create_with_ranges(sys, props, num_props, num_frames, &one, ranges, num_ranges);
             if (!q) { destroy_plan(root); return nullptr; }
             root->multi->peers.push_back(q);
         }
@@ -523,11 +542,29 @@ mdgpu_plan* mdgpu_plan_create(const mdgpu_system_desc_t* sys, const mdgpu_proper
                 da[0].radius_min = d.ref_within_min; da[0].radius_max = d.ref_within_radius; da[0].has_and = d.com_args & 1u;
                 da[0].and_idx = d.idx[2]; da[0].and_count = d.idx_count[2];
             }
-            for (int k = 0; k < 4; ++k) if (da[k].radius_max > 0.0f && pr.op != MDGPU_OP_WITHIN_COUNT) {
+            for (int k = 0; k < 4; ++k) {
+                const mdgpu_range_arg_t* rng = range_of[i][k];
+                const bool range = rng != nullptr;
+                if (!range && !(da[k].radius_max > 0.0f && pr.op != MDGPU_OP_WITHIN_COUNT)) continue;
                 const bool ok_op = (pr.op == MDGPU_OP_RDF && k < 2) || (pr.op == MDGPU_OP_SDF && k == 1) || (pr.is_density() && k == 0) ||
                                    ((pr.op == MDGPU_OP_DISTANCE || pr.op == MDGPU_OP_ANGLE || pr.op == MDGPU_OP_DIHEDRAL) && !d.num_structures) || (pr.op == MDGPU_OP_COM && k == 0) ||
-                                   ((pr.op == MDGPU_OP_DISTANCE_MIN || pr.op == MDGPU_OP_DISTANCE_MAX) && k < 2);
+                                   ((pr.op == MDGPU_OP_DISTANCE_MIN || pr.op == MDGPU_OP_DISTANCE_MAX) && k < 2) || (range && pr.op == MDGPU_OP_WITHIN_COUNT && k == 0);
                 if (!ok_op) return bail(MDGPU_ERR_UNSUPPORTED, "property '" + pr.name + "': a dynamic selection is not lowered as argument " + std::to_string(k) + " of this procedure");
+                if (range) {
+                    if (da[k].radius_min != 0.0f || da[k].radius_max != 0.0f || (pr.op == MDGPU_OP_WITHIN_COUNT && (pr.cutoff_min != 0.0f || pr.cutoff_max != 0.0f)))
+                        return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': argument " + std::to_string(k) + " has both a radius and a coordinate range");
+                    if (!pr.h_idx[k].empty()) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': a coordinate range takes no selection in idx[" + std::to_string(k) + "]");
+                    for (int c = 0; c < 3; ++c)
+                        if (!(rng->lo[c] <= rng->hi[c])) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': invalid coordinate range (lower bound above the upper one, or NaN)");
+                    Prop::DynArg& dy = pr.dyn[k];
+                    dy.on = true; dy.range = true; dy.has_and = da[k].has_and != 0;
+                    for (int c = 0; c < 3; ++c) { dy.lo[c] = rng->lo[c]; dy.hi[c] = rng->hi[c]; }
+                    if (dy.has_and) {   // the static side as an index list: the mark kernel tests only these atoms
+                        for (size_t j = 0; j < da[k].and_count; ++j) if (da[k].and_idx[j] < 0 || (size_t)da[k].and_idx[j] >= sys->num_atoms) return bail(MDGPU_ERR_INVALID_ARG, "property '" + pr.name + "': atom index out of range");
+                        if (da[k].and_count && dy.d_and_idx.upload(da[k].and_idx, da[k].and_count) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (selection list)");
+                    }
+                    continue;
+                }
                 if (da[k].radius_min < 0.0f || da[k].radius_max < da[k].radius_min) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': The supplied radius range is invalid");   // :2654
                 pr.dyn[k].on = true; pr.dyn[k].rmin = da[k].radius_min; pr.dyn[k].rmax = da[k].radius_max;
                 if (da[k].has_and && !take_and_mask(pr, pr.dyn[k].d_and_mask, da[k].and_idx, da[k].and_count)) return nullptr;
@@ -618,7 +655,8 @@ mdgpu_plan* mdgpu_plan_create(const mdgpu_system_desc_t* sys, const mdgpu_proper
             if (len > 1000000) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': The size produced by the operation is " + std::to_string(len) + ", which exceeds the upper limit of 1'000'000");   // :4056
             e = set_temporal(pr, num_frames, len);
             break; }
-        case MDGPU_OP_WITHIN_COUNT:   // count(within(radius, selection)); an empty selection is valid (nothing is within reach of nothing)
+        case MDGPU_OP_WITHIN_COUNT:   // count(within(radius, selection)); an empty selection is valid (nothing is within reach of nothing). count(<range>): dyn[0]
+            if (pr.dyn[0].range) { e = set_temporal(pr, num_frames, 1); break; }
             if (!(pr.cutoff_max > 0.0f)) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': The supplied radius is negative or zero, please supply a positive value");   // :2528
             if (pr.cutoff_min < 0.0f || pr.cutoff_max < pr.cutoff_min) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': The supplied radius range is invalid");          // :2654
             e = set_temporal(pr, num_frames, 1);
@@ -830,11 +868,14 @@ static size_t rdf_list_stride(const mdgpu_plan* p, const Prop& pr, const mdgpu_u
     return std::min<size_t>(nn, 125) * (pr.dyn[1].on ? std::max<size_t>(p->num_atoms / 4, 1024) : pr.h_idx[1].size()) + 1024;
 }
 
-// the scratch of one within() query over a selection of n_sel atoms; `list`: with the per-frame index list of a dynamic argument
-static int alloc_within(mdgpu_plan* p, WithinScratch& w, size_t n_sel, uint32_t cap, bool list) {
-    CUDA_TRY(w.d_geom.alloc(p->B)); CUDA_TRY(w.d_aabb.alloc((size_t)6 * p->B));
-    CUDA_TRY(w.trg.alloc(p->B, (uint32_t)p->num_atoms, cap));
-    CUDA_TRY(w.ref.alloc(p->B, (uint32_t)std::max<size_t>(n_sel, 1), cap));
+// the scratch of one within() query over a selection of n_sel atoms; `list`: with the per-frame index list of a dynamic argument.
+// A coordinate range (`cells` false) needs no grid and no cell lists: only the marks and the list.
+static int alloc_within(mdgpu_plan* p, WithinScratch& w, size_t n_sel, uint32_t cap, bool list, bool cells = true) {
+    if (cells) {
+        CUDA_TRY(w.d_geom.alloc(p->B)); CUDA_TRY(w.d_aabb.alloc((size_t)6 * p->B));
+        CUDA_TRY(w.trg.alloc(p->B, (uint32_t)p->num_atoms, cap));
+        CUDA_TRY(w.ref.alloc(p->B, (uint32_t)std::max<size_t>(n_sel, 1), cap));
+    }
     CUDA_TRY(w.d_flags.alloc((size_t)p->B * p->num_atoms));
     if (list) { CUDA_TRY(w.d_idx.alloc((size_t)p->B * p->num_atoms)); CUDA_TRY(w.d_n.alloc(p->B)); }
     return 0;
@@ -852,7 +893,9 @@ static int build_slot(mdgpu_plan* p, Slot& s, const mdgpu_unitcell_t* first_cell
     s.ps.resize(p->props.size());
     for (size_t i = 0; i < p->props.size(); ++i) {
         Prop& pr = p->props[i]; PropScratch& ps = s.ps[i];
-        for (int k = 0; k < 4; ++k) if (pr.dyn[k].on) { const int rc = alloc_within(p, ps.within[k], pr.h_idx[k].size(), cap, true); if (rc) return rc; }
+        for (int k = 0; k < 4; ++k) if (pr.dyn[k].on) {
+            const int rc = alloc_within(p, ps.within[k], pr.h_idx[k].size(), cap, pr.op != MDGPU_OP_WITHIN_COUNT, !pr.dyn[k].range); if (rc) return rc;
+        }
         // an argument that is an array of selections: one position per selection
         for (int k = 0; k < 2; ++k) if (!pr.h_goff[k].empty()) CUDA_TRY(ps.d_gpos[k].alloc((size_t)p->B * (pr.h_goff[k].size() - 1) * 3));
         if (pr.needs_cells() && pr.share_trg < 0) {
@@ -875,7 +918,7 @@ static int build_slot(mdgpu_plan* p, Slot& s, const mdgpu_unitcell_t* first_cell
             CUDA_TRY(ps.d_sdf_xyzw.alloc((size_t)p->B * (pr.n_struct + 1) * pr.struct_size));
             CUDA_TRY(ps.d_sdf_ref0.alloc((size_t)p->B * 20));
             CUDA_TRY(ps.d_sdf_mats.alloc((size_t)p->B * pr.n_struct * 32));
-        } else if (pr.op == MDGPU_OP_WITHIN_COUNT) {
+        } else if (pr.op == MDGPU_OP_WITHIN_COUNT && !pr.dyn[0].on) {
             const int rc = alloc_within(p, ps.within[0], pr.h_idx[0].size(), cap, false); if (rc) return rc;
         } else if (pr.op == MDGPU_OP_POROSITY) {
             CUDA_TRY(ps.d_poro_xyzr.alloc((size_t)PORO_FRAMES * pr.h_idx[0].size())); CUDA_TRY(ps.d_poro_hdr.alloc(PORO_FRAMES));
@@ -912,8 +955,8 @@ static int ensure_slots(mdgpu_plan* p, const mdgpu_unitcell_t* first_cell, bool 
             };
             for (auto& pr : p->props) {
                 if (pr.needs_cells()) grid((double)pr.cutoff_max, pr.cutoff_max);
-                if (pr.op == MDGPU_OP_WITHIN_COUNT) grid(within_cell_ext(pr.cutoff_max), pr.cutoff_max);
-                for (auto& dy : pr.dyn) if (dy.on) grid(within_cell_ext(dy.rmax), dy.rmax);
+                if (pr.op == MDGPU_OP_WITHIN_COUNT && !pr.dyn[0].on) grid(within_cell_ext(pr.cutoff_max), pr.cutoff_max);
+                for (auto& dy : pr.dyn) if (dy.on && !dy.range) grid(within_cell_ext(dy.rmax), dy.rmax);
             }
             cap = (uint32_t)std::min<uint64_t>(need, 1u << 26);
         }
@@ -965,6 +1008,17 @@ static WithinArgs enqueue_within(mdgpu_plan* p, Slot& s, WithinScratch& w, const
     return a;
 }
 
+// a coordinate range of every frame of the batch: the arguments of launch_range_list / launch_range_count (frames in the full atom space:
+// a range consumer makes host ingest copy whole frames)
+static RangeArgs range_args(const mdgpu_plan* p, const Prop::DynArg& dy, WithinScratch& w, const BatchFrames& fr) {
+    RangeArgs a{};
+    a.frames = fr;
+    for (int c = 0; c < 3; ++c) { a.lo[c] = dy.lo[c]; a.hi[c] = dy.hi[c]; }
+    a.has_and = dy.has_and ? 1u : 0u; a.and_idx = dy.d_and_idx.get(); a.n_and = (uint32_t)dy.d_and_idx.size();
+    a.num_atoms = (uint32_t)p->num_atoms; a.flags = w.d_flags.get();
+    return a;
+}
+
 // what `launch` enqueues on `st`, timed as one TimedLaunch of `kind` when kernel timing is enabled
 template <typename F> static void timed_launch(mdgpu_plan* p, cudaStream_t st, int kind, F&& launch) {
     TimedLaunch tl{ nullptr, nullptr, kind };
@@ -994,11 +1048,12 @@ static int enqueue_batch(mdgpu_plan* p, Slot& s, const BatchFrames& fr, uint32_t
         DynSel dsel[4];
         for (int k = 0; k < 4; ++k) {   // dynamic arguments first: within([min:]max, idx[k]) [and mask] of every frame of the batch -> ascending per-frame lists
             dsel[k] = DynSel{ nullptr, nullptr, 0 };
-            if (!pr.dyn[k].on) continue;
+            if (!pr.dyn[k].on || pr.op == MDGPU_OP_WITHIN_COUNT) continue;   // count() of a range reads the marks itself (below)
             auto& w = ps.within[k];
+            dsel[k] = DynSel{ w.d_idx.get(), w.d_n.get(), (uint32_t)p->num_atoms };
+            if (pr.dyn[k].range) { launch_range_list(range_args(p, pr.dyn[k], w, fr), B, p->sm_count, w.d_idx.get(), w.d_n.get(), s.stream); continue; }
             const WithinArgs wa = enqueue_within(p, s, w, fr, all_pbc, didx[k], pr.h_idx[k].size(), pr.dyn[k].rmin, pr.dyn[k].rmax, pr.dyn[k].d_and_mask.get(), frame0);
             launch_within_list(wa, B, tri, p->sm_count, w.d_idx.get(), w.d_n.get(), s.stream);
-            dsel[k] = DynSel{ w.d_idx.get(), w.d_n.get(), (uint32_t)p->num_atoms };
         }
         if (pr.needs_cells() && pr.share_trg < 0) {
             // target groups: the target points are the groups' centres of mass, an AoS stream, j = position index (compute_rdf :5299-5301);
@@ -1079,6 +1134,7 @@ static int enqueue_batch(mdgpu_plan* p, Slot& s, const BatchFrames& fr, uint32_t
             timed_launch(p, s.stream, 2, [&] { launch_density(a, B, s.stream); });
             break; }
         case MDGPU_OP_WITHIN_COUNT: {
+            if (pr.dyn[0].on) { launch_range_count(range_args(p, pr.dyn[0], ps.within[0], fr), B, p->sm_count, pr.d_temporal.get(), frame0, s.stream); break; }
             WithinArgs a = enqueue_within(p, s, ps.within[0], fr, all_pbc, didx[0], pr.h_idx[0].size(), pr.cutoff_min, pr.cutoff_max, pr.d_and_mask.get(), frame0);
             a.out = pr.d_temporal.get();
             launch_within_count(a, B, tri, p->sm_count, s.stream);

@@ -192,7 +192,7 @@ __global__ void k_arg_com(BatchFrames fr, const mdgpu_unitcell_t* __restrict__ c
 }
 
 void launch_arg_com(const BatchFrames& fr, const mdgpu_unitcell_t* d_cells, const int32_t* d_idx, uint32_t count, const float* d_mass, float* d_out, int arg, cudaStream_t s, DynSel dyn) {
-    if (!fr.count || !count) return;
+    if (!fr.count || (!count && !dyn.n)) return;   // a coordinate range has no static list: its per-frame list is all there is
     k_arg_com<<<fr.count, 32, 0, s>>>(fr, d_cells, d_idx, count, d_mass, d_out, arg, dyn);
     note_launch("k_arg_com", s);
 }

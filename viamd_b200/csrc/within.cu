@@ -1,4 +1,4 @@
-// within.cu — dynamic selections, first consumer: count(within(radius, selection)) evaluated per frame.
+// within.cu — dynamic selections: within(radius, selection) and the coordinate ranges within_x / _y / _z / _xyz, evaluated per frame.
 //
 // Replaces _within_expl_flt + within_float_cb (reference md_script_functions.inl:2478-2533) over the system-wide cell list of
 // get_spatial_acc (:734-760: every atom of the system, cell extent ceil(radius / 6) * 6), and _count (:2868) on the result:
@@ -128,6 +128,58 @@ void launch_within_count(const WithinArgs& a, int B, bool tri, int sm_count, cud
     if (B <= 0) return;
     launch_mark(a, B, tri, sm_count, s);
     k_within_count<<<B, 256, 0, s>>>(a);
+    note_launch("k_within_count", s);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Coordinate ranges within_x / _y / _z / _xyz(...) (coordinate_range md_script_functions.inl:2394-2476, the form outside an `in` context):
+// atom i is selected iff lo <= p[i] <= hi on all three axes, on the frame's raw coordinates. Unconstrained axes come as [-FLT_MAX, FLT_MAX] and
+// are compared like the others, so a NaN or infinite coordinate is never selected. No atom is removed afterwards: the compaction and the count
+// run with n_sel = 0. One frame per block row; with a static `and` side only its atoms are tested (the flags were zeroed first), otherwise
+// every atom's flag is written.
+// ---------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) k_range_mark(RangeArgs a) {
+    const int f = blockIdx.y;
+    const float* __restrict__ x = a.frames.xyz + (size_t)f * a.frames.frame_stride;
+    const float* __restrict__ y = x + a.frames.axis_stride;
+    const float* __restrict__ z = y + a.frames.axis_stride;
+    uint8_t* __restrict__ flags = a.flags + (size_t)f * a.num_atoms;
+    const uint32_t n = a.has_and ? a.n_and : a.num_atoms;
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x) {
+        const uint32_t i = a.has_and ? (uint32_t)a.and_idx[j] : j;
+        const float px = x[i], py = y[i], pz = z[i];
+        const bool in = a.lo[0] <= px && px <= a.hi[0] && a.lo[1] <= py && py <= a.hi[1] && a.lo[2] <= pz && pz <= a.hi[2];
+        if (!a.has_and) flags[i] = in ? 1 : 0;
+        else if (in) flags[i] = 1;
+    }
+}
+
+// the marks of a batch, and the WithinArgs under which k_within_compact / k_within_count read them
+static WithinArgs range_mark(const RangeArgs& a, int B, int sm_count, cudaStream_t s) {
+    const uint32_t n = a.has_and ? a.n_and : a.num_atoms;
+    if (a.has_and) cudaMemsetAsync(a.flags, 0, (size_t)B * a.num_atoms, s);
+    if (n) {
+        const unsigned per_frame = (unsigned)min((n + 255u) / 256u, (uint32_t)max(1, (8 * sm_count) / max(B, 1)));
+        k_range_mark<<<dim3(per_frame, (unsigned)B), 256, 0, s>>>(a);
+        note_launch("k_range_mark", s);
+    }
+    WithinArgs w{};
+    w.num_atoms = a.num_atoms; w.flags = a.flags;   // n_sel = 0, no and_mask: the marks are the selection
+    return w;
+}
+
+void launch_range_list(const RangeArgs& a, int B, int sm_count, int32_t* d_dyn_idx, uint32_t* d_dyn_n, cudaStream_t s) {
+    if (B <= 0) return;
+    const WithinArgs w = range_mark(a, B, sm_count, s);
+    k_within_compact<<<B, 256, 0, s>>>(w, d_dyn_idx, d_dyn_n);
+    note_launch("k_within_compact", s);
+}
+
+void launch_range_count(const RangeArgs& a, int B, int sm_count, float* d_out, uint32_t frame0, cudaStream_t s) {
+    if (B <= 0) return;
+    WithinArgs w = range_mark(a, B, sm_count, s);
+    w.out = d_out; w.frame0 = frame0;
+    k_within_count<<<B, 256, 0, s>>>(w);
     note_launch("k_within_count", s);
 }
 

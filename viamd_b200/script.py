@@ -11,6 +11,8 @@ Supported statements:  ident = proc(args);   with proc in
     porosity(sel)                                                        (needs System.radius)
 Selections (evaluated once, statically, to ascending atom index lists — md_script.c:5492-5524):
     all | element('O') | name('C2*') | resname('SOL') | atom(a:b) | residue(a:b) | `and` / `or` / `not` of these
+Dynamic selections (evaluated per frame on the device), alone or `static and ...` in either order, where a consumer accepts them:
+    within([min:]max, sel) | within_x(a:b) | within_y(a:b) | within_z(a:b) | within_xyz(a:b, c:d, e:f)
 `residue(a:b)` used as the first argument of sdf() yields one structure per residue (bitfield array semantics).
 """
 from __future__ import annotations
@@ -28,6 +30,9 @@ _TOK = re.compile(r"\s*(?:(\d+\.\d*|\.\d+|\d+)|([A-Za-z_][A-Za-z_0-9]*)|'([^']*)
 
 class ScriptError(ValueError):
     pass
+
+
+_DYNAMIC = ("within", "within_x", "within_y", "within_z", "within_xyz")   # selections whose atoms depend on the frame's coordinates (FLAG_DYNAMIC)
 
 
 def _tokens(src: str):
@@ -57,7 +62,7 @@ class _Parser:
 
     # ---- selections -> boolean masks
     _static_seen = False
-    _within = None   # (min, max, selection) of the one dynamic within() met while parsing a selection expression, see dyn_selection()
+    _within = None   # the one dynamic selection met while parsing a selection expression, see dyn_arg(): ("within", min, max, selection) | ("range", lo, hi)
 
     def sel_or(self):
         m = self.sel_and()
@@ -81,14 +86,26 @@ class _Parser:
             return m
         return self.sel_atom()
 
-    def dyn_selection(self):
-        """`within([min:]max, sel)` or `static and within(...)` (either order) -> (min, max, within's selection, static side's atoms or None);
-        the dynamic part is evaluated per frame on the device, the static side becomes its AND mask (_and md_script_functions.inl:1975)"""
+    def dyn_arg(self):
+        """`within([min:]max, sel)` or a coordinate range within_x / _y / _z / _xyz(...), alone or `static and ...` (either order) -> api.Within /
+        api.Range; the dynamic part is evaluated per frame on the device, the static side becomes its AND side (_and md_script_functions.inl:1975)"""
         self._within = None; self._static_seen = False
         m = self.sel_or()
         if self._within is None: raise ScriptError("a within(...) expression was expected")
-        lo, hi, sel = self._within; self._within = None
-        return lo, hi, sel, (np.nonzero(m)[0].astype(np.int32) if self._static_seen else None)
+        w = self._within; self._within = None
+        cand = np.nonzero(m)[0].astype(np.int32) if self._static_seen else None
+        return api.Range(w[1], w[2], cand) if w[0] == "range" else api.Within(w[2], w[3], w[1], cand)
+
+    def frange(self):
+        """a:b | a: | :b | : (the range literal, md_script.c) -> (lo, hi) of the frange the front end hands a procedure that takes one: bounds of a
+        float range as floats with open ends at -FLT_MAX / FLT_MAX; an integer range keeps INT32_MIN / INT32_MAX for open ends and is cast
+        bound by bound to float (_cast_irng_to_frng md_script_functions.inl:4378)"""
+        lo = hi = None; is_float = False
+        if self.peek()[0] == "num": t = self.next()[1]; lo = float(t); is_float |= "." in t
+        self.expect("ch", ":")
+        if self.peek()[0] == "num": t = self.next()[1]; hi = float(t); is_float |= "." in t
+        if is_float: return (-api.FLT_MAX if lo is None else float(np.float32(lo)), api.FLT_MAX if hi is None else float(np.float32(hi)))
+        return (float(np.float32(-2 ** 31 if lo is None else int(lo))), float(np.float32(2 ** 31 - 1 if hi is None else int(hi))))
 
     def _range(self, count):
         """a | a:b | : (1-based inclusive, as in md_script) -> python slice bounds (0-based, exclusive end)"""
@@ -108,11 +125,19 @@ class _Parser:
         if tok[0] != "id":
             raise ScriptError(f"unexpected token {tok[1]!r} in selection")
         f = tok[1]
-        if f == "within":   # only inside dyn_selection(): stands for "every atom" in the static mask, the device supplies the real set
-            if self._within is not None: raise ScriptError("one within() per expression")
-            self.expect("ch", "("); lo, hi = self.radius(); self.expect("ch", ",")
-            seen = self._static_seen; sel = self.selection(); self._static_seen = seen; self.expect("ch", ")")   # within's own argument is not the static side; FLAG_FLATTEN (:673): an array of selections is their union
-            self._within = (lo, hi, sel); return np.ones(n, bool)
+        if f in _DYNAMIC:   # only inside dyn_arg(): stands for "every atom" in the static mask, the device supplies the real set
+            if self._within is not None: raise ScriptError("one dynamic selection (within, within_x / _y / _z / _xyz) per expression")
+            self.expect("ch", "(")
+            if f == "within":
+                lo, hi = self.radius(); self.expect("ch", ",")
+                seen = self._static_seen; sel = self.selection(); self._static_seen = seen; self.expect("ch", ")")   # within's own argument is not the static side; FLAG_FLATTEN (:673): an array of selections is their union
+                self._within = ("within", lo, hi, sel); return np.ones(n, bool)
+            lo, hi = [-api.FLT_MAX] * 3, [api.FLT_MAX] * 3   # coordinate_range :2394: unconstrained axes are [-FLT_MAX, FLT_MAX]
+            for c in (range(3) if f == "within_xyz" else ["xyz".index(f[-1])]):
+                if c and f == "within_xyz": self.expect("ch", ",")
+                lo[c], hi[c] = self.frange()
+            self.expect("ch", ")")
+            self._within = ("range", lo, hi); return np.ones(n, bool)
         self._static_seen = True
         if f == "all": return np.ones(n, bool)
         self.expect("ch", "(")
@@ -142,7 +167,9 @@ class _Parser:
         raise ScriptError(f"unsupported selection '{f}'")
 
     def selection(self) -> np.ndarray:
-        return np.nonzero(self.sel_or())[0].astype(np.int32)
+        m = self.sel_or()
+        if self._within is not None: raise ScriptError("a dynamic selection is not lowered as this argument")
+        return np.nonzero(m)[0].astype(np.int32)
 
     def structures(self) -> np.ndarray:
         """first argument of sdf(): residue(a:b) -> one structure per residue; otherwise a single structure"""
@@ -192,7 +219,7 @@ class _Parser:
                 if depth == 0: return False
                 depth -= 1
             elif t == ("ch", ",") and depth == 0: return False
-            elif t == ("id", "within"): return True
+            elif t[0] == "id" and t[1] in _DYNAMIC: return True
         return False
 
     def groups_or_selection(self):
@@ -208,9 +235,7 @@ class _Parser:
 
     def sel_or_within(self, single=False):
         """a selection argument that may be a dynamic one: index array, or api.Within for `within([min:]max, sel)` [and static]"""
-        if self._has_within_before_comma():
-            lo, hi, sel, cand = self.dyn_selection()
-            return api.Within(hi, sel, lo, cand)
+        if self._has_within_before_comma(): return self.dyn_arg()
         return self.single_selection() if single else self.selection()
 
     def number(self) -> float:
@@ -263,19 +288,21 @@ class _Parser:
         proc = self.expect("id")[1]; self.expect("ch", "(")
         self.arg_meta = []   # how each argument of distance / angle / dihedral was written (index()): decides its meaning inside `in` contexts
         if proc == "rdf":
-            wr = None
-            if self._has_within_before_comma():   # dynamic reference set: within([min:]max, selection), optionally `and` a static selection
-                wlo, wr, wsel, wand = self.dyn_selection()
-            grp = self.groups() if wr is None else None
-            ref = None if (grp is not None or wr is not None) else self.selection()
+            wr = rr = None
+            if self._has_within_before_comma():   # dynamic reference set: within([min:]max, selection) or a coordinate range, optionally `and` a static selection
+                d = self.dyn_arg()
+                if isinstance(d, api.Range): rr = d
+                else: wlo, wr, wsel, wand = d.radius_min, d.radius, d.sel, d.and_idx
+            grp = self.groups() if (wr is None and rr is None) else None
+            ref = rr if rr is not None else (None if (grp is not None or wr is not None) else self.selection())
             self.expect("ch", ",")
             trg = self.sel_or_within() if self._has_within_before_comma() else self.groups_or_selection()   # an array of selections as target: one centre of mass each
             self.expect("ch", ",")
             a = self.number(); lo, hi = 0.0, a
             if self.peek() == ("ch", ":"):
                 self.next(); lo, hi = a, self.number()
-            if wr is not None and isinstance(trg, list): raise ScriptError("a dynamic reference set with an array of selections as target is not lowered")
-            if wr is not None: p = api.rdf(ident, api.Within(wr, wsel, wlo, wand), trg, hi, lo) if isinstance(trg, api.Within) else api.rdf_within(ident, wr, wsel, trg, hi, lo, wlo, wand)
+            if (wr is not None or rr is not None) and isinstance(trg, list): raise ScriptError("a dynamic reference set with an array of selections as target is not lowered")
+            if wr is not None: p = api.rdf(ident, api.Within(wr, wsel, wlo, wand), trg, hi, lo) if isinstance(trg, (api.Within, api.Range)) else api.rdf_within(ident, wr, wsel, trg, hi, lo, wlo, wand)
             else: p = api.rdf_com(ident, grp, trg, hi, lo) if grp is not None else api.rdf(ident, ref, trg, hi, lo)
         elif proc == "sdf":
             st = self.structures(); self.expect("ch", ","); trg = self.sel_or_within(); self.expect("ch", ","); c = self.number()
@@ -293,10 +320,10 @@ class _Parser:
             a = self.groups_or_selection(); self.expect("ch", ","); b = self.selection(); self.expect("ch", ","); c = self.number()
             if self.peek() == ("ch", ","): raise ScriptError("Could not find matching procedure 'contact_count' which takes four arguments")
             p = api.contact_count(ident, a if isinstance(a, list) else [a], b, c, self.sys, 4)
-        elif proc == "count":   # count(within(radius, selection)): the one dynamic selection the device path evaluates
-            if not self._has_within_before_comma(): raise ScriptError("count() is lowered for within(radius, selection) expressions only")
-            rlo, r, sel, cand = self.dyn_selection()
-            p = api.count_within(ident, r, sel, rlo, cand)
+        elif proc == "count":   # count(<dynamic selection>): the selection is evaluated per frame on the device
+            if not self._has_within_before_comma(): raise ScriptError("count() is lowered for within(...) and within_x / _y / _z / _xyz(...) expressions only")
+            d = self.dyn_arg()
+            p = api.count_range(ident, d) if isinstance(d, api.Range) else api.count_within(ident, d.radius, d.sel, d.radius_min, d.and_idx)
         elif proc in ("coord_x", "coord_y", "coord_z"):
             a = self.index()   # an array of selections: one value per selection (its centre of mass, coordinate_extract :1503)
             p = api.coord(ident, "xyz".index(proc[-1]), a if isinstance(a, list) else ([a] if np.ndim(a) == 0 else a))
