@@ -155,6 +155,10 @@ typedef enum mdgpu_op {
  *              md_util.c:2588-2592) whose two values stay 0. Row f holds md_backbone_angles_t[num_structures] = (phi, psi) pairs in radians:
  *              phi = dihedral(C', N, CA, C), psi = dihedral(N, CA, C, N') with md_util_min_image_vec3 on the bond vectors, as `dihedral` evaluates.
  *   RMSD     : idx[0] = the atoms of the (flattened) selection; needs the initial frame and, to make molecules whole, the bond connectivity.
+ *              With num_structures = n > 0 the statement was `rmsd(x) in <n contexts>` (evaluate_context md_script.c:3418): idx[0] holds n groups
+ *              back to back, group c = the atoms of (flattened x AND context c), delimited by structure_offsets[n+1], or `structure_size` atoms each
+ *              when that pointer is NULL (as for rdf). Groups may be empty (their value is 0) and an atom may be in several groups. The property
+ *              is [F, n] with the per-frame aggregates; each group is fitted on its own, exactly as the single-selection form fits its selection.
  *   POROSITY : idx[0] = the atoms of the (flattened) selection, ascending; needs mdgpu_system_desc_t.atom_radius. Per frame, value_range [0, 1]:
  *              0 when the frame's cell is triclinic or the selection is empty (as the reference, which logs an error there). Otherwise
  *              xyzr = (x, y, z, radius) of the selected atoms in index order; com = md_util_com_compute_vec4(xyzr, 0, n, cell) (the trigonometric

@@ -487,7 +487,13 @@ def backbone_angles(name, five):
 
 def rmsd(name, idx):
     """rmsd(selection): mass-weighted RMSD of the selection's atoms against the initial frame after wrap, bond-walk unwrap and an optimal
-    rotation (_rmsd md_script_functions.inl:4287). Needs System.conn_offset / conn_idx to make molecules whole, as the reference does."""
+    rotation (_rmsd md_script_functions.inl:4287). Needs System.conn_offset / conn_idx to make molecules whole, as the reference does.
+    A LIST of index arrays is `rmsd(x) in <contexts>`: one group per context (the atoms of x AND the context), each fitted on its own -> [F, n];
+    an empty group evaluates to 0."""
+    if isinstance(idx, list):
+        g = [np.asarray(x, np.int32) for x in idx]
+        off = np.zeros(len(g) + 1, np.uint32); off[1:] = np.cumsum([len(x) for x in g])
+        return Property(name, OP_RMSD, [np.concatenate(g).astype(np.int32) if off[-1] else np.zeros(0, np.int32)], num_structures=len(g), structure_offsets=off)
     return Property(name, OP_RMSD, [np.asarray(idx, np.int32)])
 
 

@@ -95,10 +95,13 @@ struct RmsdArgs {                    // rmsd(selection) against the initial fram
     const float* pos;                // plane() of an ARRAY of selections: [B][n][3] centres of mass, the n positions (idx unused); else null
     const int2* unwrap_pairs; uint32_t n_unwrap;
     float4* scratch_xyzw;            // [B][2][n]
-    float* out;                      // [num_frames]
+    float* out;                      // [num_frames], or [num_frames][n_groups] for groups
     uint32_t frame0;
+    // rmsd(selection) in <contexts>: n_groups groups of idx[0] (CSR soff); group g walks the n pairs unwrap_pairs[first ..) of group_pairs[g] = (first, n)
+    const uint32_t* soff; const uint2* group_pairs; uint32_t n_groups;
 };
 void launch_rmsd(const RmsdArgs& a, int B, cudaStream_t s);
+void launch_rmsd_groups(const RmsdArgs& a, int B, cudaStream_t s);   // one value per group and frame (k_rmsd_groups)
 void launch_plane(const RmsdArgs& a, int B, cudaStream_t s);   // plane(selection): out is [num_frames][4], scratch [B][n], init_xyz unused
 
 // within.cu — count(within(radius, selection))

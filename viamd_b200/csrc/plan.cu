@@ -138,6 +138,7 @@ struct Prop {
     std::vector<float> agg_mean, agg_var, agg_ext;   // len > 1: per-frame mean / population variance / (min, max) (md_script_aggregate_t)
     // sdf statics
     DevBuf<int2> d_unwrap; uint32_t n_unwrap = 0;
+    DevBuf<uint2> d_group_pairs;   // rmsd in contexts: per group (first pair in d_unwrap, pair count)
     // density statics (from the initial frame's cell)
     float rc = 0, re = 0, inv_ext = 0, min_point = 0; double dens_factor = 0;
     // results: `values` is the default storage; mdgpu_plan_bind_property_storage points vptr (and the aggregate rows) at the caller's arrays
@@ -731,10 +732,31 @@ mdgpu_plan* mdgpu_plan_create_with_ranges(const mdgpu_system_desc_t* sys, const 
             break;
         case MDGPU_OP_RMSD: {   // an empty selection is valid and evaluates to 0 (_rmsd :4311, :4336-4338)
             std::vector<int2> pairs;   // without bonds md_util_unwrap_vec4 fails and its result is ignored (:4327): nothing is unwrapped
-            build_unwrap_pairs(pairs, pr.h_idx[0].size(), p->conn_off, p->conn_idx);
+            if (!pr.n_struct) {
+                build_unwrap_pairs(pairs, pr.h_idx[0].size(), p->conn_off, p->conn_idx);
+                pr.n_unwrap = (uint32_t)pairs.size();
+                e = pr.d_unwrap.upload(pairs.data(), pairs.size());
+                if (e == cudaSuccess) e = set_temporal(pr, num_frames, 1);
+                break;
+            }
+            // `rmsd(x) in <n contexts>`: n groups of idx[0], one value each. A group's unwrap pairs depend on its size only: built once per size.
+            { const std::string er = take_structures(pr, d, "rmsd '" + pr.name + "'"); if (!er.empty()) return bail(MDGPU_ERR_INVALID_ARG, er); }
+            std::map<uint32_t, uint2> by_size; std::vector<uint2> gp(pr.n_struct);
+            for (size_t g = 0; g < pr.n_struct; ++g) {
+                const uint32_t sz = pr.h_soff[g + 1] - pr.h_soff[g];
+                auto it = by_size.find(sz);
+                if (it == by_size.end()) {
+                    std::vector<int2> one; build_unwrap_pairs(one, sz, p->conn_off, p->conn_idx);
+                    it = by_size.emplace(sz, make_uint2((uint32_t)pairs.size(), (uint32_t)one.size())).first;
+                    pairs.insert(pairs.end(), one.begin(), one.end());
+                }
+                gp[g] = it->second;
+            }
             pr.n_unwrap = (uint32_t)pairs.size();
             e = pr.d_unwrap.upload(pairs.data(), pairs.size());
-            if (e == cudaSuccess) e = set_temporal(pr, num_frames, 1);
+            if (e == cudaSuccess) e = pr.d_group_pairs.upload(gp.data(), gp.size());
+            if (e == cudaSuccess) e = pr.d_soff.upload(pr.h_soff.data(), pr.h_soff.size());
+            if (e == cudaSuccess) e = set_temporal(pr, num_frames, pr.n_struct);
             break; }
         default:
             return bail(MDGPU_ERR_UNSUPPORTED, "property '" + pr.name + "': unsupported operation " + std::to_string(pr.op));
@@ -1186,7 +1208,10 @@ static int enqueue_batch(mdgpu_plan* p, Slot& s, const BatchFrames& fr, uint32_t
             a.frames = fr; a.cells = s.d_cells.get(); a.init_xyz = dinit; a.init_axis_stride = init_as; a.mass = dmass;
             a.idx = didx[0]; a.n = (uint32_t)pr.h_idx[0].size(); a.unwrap_pairs = pr.d_unwrap.get(); a.n_unwrap = pr.n_unwrap;
             a.scratch_xyzw = ps.d_sdf_xyzw.get(); a.out = pr.d_temporal.get(); a.frame0 = frame0;
-            launch_rmsd(a, B, s.stream);
+            if (pr.n_struct) {   // one value per context
+                a.soff = pr.d_soff.get(); a.group_pairs = pr.d_group_pairs.get(); a.n_groups = (uint32_t)pr.n_struct;
+                launch_rmsd_groups(a, B, s.stream);
+            } else launch_rmsd(a, B, s.stream);
             break; }
         case MDGPU_OP_DISTANCE_MIN: case MDGPU_OP_DISTANCE_MAX: {   // both evaluate md_util_min_distance (md_script_functions.inl:3904, 3944)
             const ArgPoints g0 = group_positions(pr, ps, 0, fr, didx[0], dmass, s.stream), g1 = group_positions(pr, ps, 1, fr, didx[1], dmass, s.stream);

@@ -516,24 +516,18 @@ MDG_D float4 pbc_wrap(float4 v, const mdgpu_unitcell_t& uc) {
     return v;
 }
 
-__global__ void __launch_bounds__(32) k_rmsd(RmsdArgs a, int B) {
-    const int f = blockIdx.x, lane = threadIdx.x;
-    if (f >= B) return;
-    const uint32_t n = a.n;
-    const mdgpu_unitcell_t uc = a.cells[f];
-    const float* x = a.frames.xyz + (size_t)f * a.frames.frame_stride;
-    float4* p0 = a.scratch_xyzw + (size_t)f * 2 * n;   // initial frame
-    float4* p1 = p0 + n;                               // current frame
-    for (uint32_t k = lane; k < n; k += 32) {           // extract_xyzw_vec4 (:966) + md_util_pbc_vec4
-        const int at = a.idx[k]; const float w = a.mass[at];
-        p0[k] = pbc_wrap(make_float4(a.init_xyz[at], a.init_xyz[a.init_axis_stride + at], a.init_xyz[2 * a.init_axis_stride + at], w), uc);
-        p1[k] = pbc_wrap(make_float4(x[at], x[a.frames.axis_stride + at], x[2 * a.frames.axis_stride + at], w), uc);
-    }
-    __syncwarp();
-    if (lane != 0) return;
+// extract_xyzw_vec4 (:966) + md_util_pbc_vec4 of atom `at` in the initial frame (-> u) and in the current frame x (-> v)
+MDG_D void rmsd_load(const RmsdArgs& a, const float* x, int at, const mdgpu_unitcell_t& uc, float4& u, float4& v) {
+    const float w = a.mass[at];
+    u = pbc_wrap(make_float4(a.init_xyz[at], a.init_xyz[a.init_axis_stride + at], a.init_xyz[2 * a.init_axis_stride + at], w), uc);
+    v = pbc_wrap(make_float4(x[at], x[a.frames.axis_stride + at], x[2 * a.frames.axis_stride + at], w), uc);
+}
+
+// The ordered part of _rmsd on n wrapped atoms: bond walk and centre of both sets, rotation from their cross-covariance, weighted deviation
+MDG_D float rmsd_fit(float4* p0, float4* p1, uint32_t n, const int2* pairs, uint32_t n_pairs, const mdgpu_unitcell_t& uc) {
     float com0[3], com1[3];
-    unwrap_com(p0, n, a.unwrap_pairs, a.n_unwrap, uc, com0);
-    unwrap_com(p1, n, a.unwrap_pairs, a.n_unwrap, uc, com1);
+    unwrap_com(p0, n, pairs, n_pairs, uc, com0);
+    unwrap_com(p1, n, pairs, n_pairs, uc, com1);
     const M3 R = extract_rotation(cross_covariance(p0, com0, p1, com1, n));
     double d_sum = 0.0, w_sum = 0.0;
     for (uint32_t k = 0; k < n; ++k) {
@@ -546,7 +540,41 @@ __global__ void __launch_bounds__(32) k_rmsd(RmsdArgs a, int B) {
         const float dd = (d[0] * d[0] + d[1] * d[1]) + d[2] * d[2];
         d_sum += (double)(w * dd); w_sum += (double)w;
     }
-    a.out[a.frame0 + f] = (float)sqrt(d_sum / w_sum);
+    return (float)sqrt(d_sum / w_sum);
+}
+
+__global__ void __launch_bounds__(32) k_rmsd(RmsdArgs a, int B) {
+    const int f = blockIdx.x, lane = threadIdx.x;
+    if (f >= B) return;
+    const uint32_t n = a.n;
+    const mdgpu_unitcell_t uc = a.cells[f];
+    const float* x = a.frames.xyz + (size_t)f * a.frames.frame_stride;
+    float4* p0 = a.scratch_xyzw + (size_t)f * 2 * n;   // initial frame
+    float4* p1 = p0 + n;                               // current frame
+    for (uint32_t k = lane; k < n; k += 32) rmsd_load(a, x, a.idx[k], uc, p0[k], p1[k]);
+    __syncwarp();
+    if (lane != 0) return;
+    a.out[a.frame0 + f] = rmsd_fit(p0, p1, n, a.unwrap_pairs, a.n_unwrap, uc);
+}
+
+// rmsd(selection) in <contexts> (evaluate_context md_script.c:3418): group g of idx[0] (soff[g] .. soff[g+1]) is (selection AND context g).
+// One thread per (group, frame), as k_sdf_fit maps structures: a context is a residue or a molecule (a few atoms), so the thread does the whole
+// ordered computation of its group. An empty group keeps the value 0 (_rmsd :4311). The unwrap pairs depend on the group's size only (the
+// local-index-as-atom quirk above): group g walks group_pairs[g] = (first pair in unwrap_pairs, pair count).
+__global__ void k_rmsd_groups(RmsdArgs a, int B) {
+    const int f = blockIdx.y;
+    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= a.n_groups) return;
+    const uint32_t beg = a.soff[g], n = a.soff[g + 1] - beg;
+    float* o = a.out + (size_t)(a.frame0 + f) * a.n_groups + g;
+    if (n == 0) { *o = 0.0f; return; }
+    const mdgpu_unitcell_t uc = a.cells[f];
+    const float* x = a.frames.xyz + (size_t)f * a.frames.frame_stride;
+    float4* p0 = a.scratch_xyzw + (size_t)f * 2 * a.n + beg;   // [B][initial, current][all groups' atoms], as k_rmsd
+    float4* p1 = p0 + a.n;
+    for (uint32_t k = 0; k < n; ++k) rmsd_load(a, x, a.idx[beg + k], uc, p0[k], p1[k]);
+    const uint2 gp = a.group_pairs[g];
+    *o = rmsd_fit(p0, p1, n, a.unwrap_pairs + gp.x, gp.y, uc);
 }
 
 // plane(selection) (_plane md_script_functions.inl:4755-4822): positions with unit weights, bond walk, plain centre, covariance
@@ -644,6 +672,12 @@ void launch_rmsd(const RmsdArgs& a, int B, cudaStream_t s) {
     if (!a.n || B <= 0) return;   // empty selection: the property stays 0 (:4311)
     k_rmsd<<<B, 32, 0, s>>>(a, B);
     note_launch("k_rmsd", s);
+}
+
+void launch_rmsd_groups(const RmsdArgs& a, int B, cudaStream_t s) {
+    if (!a.n_groups || B <= 0) return;
+    k_rmsd_groups<<<dim3((a.n_groups + 63) / 64, (unsigned)B), 64, 0, s>>>(a, B);
+    note_launch("k_rmsd_groups", s);
 }
 
 void launch_sdf(const SdfArgs& a, int B, bool tri, cudaStream_t s) {

@@ -332,6 +332,7 @@ class _Parser:
         elif proc == "plane":
             p = api.plane(ident, self.groups_or_selection())   # an array of selections: the plane through their centres of mass
         elif proc == "rmsd":
+            ctx_relative = self._arg_mentions(("atom", "residue"))   # inside `in` contexts these count from the context's first atom / residue: shim only
             p = api.rmsd(ident, self.selection())   # an array of selections is flattened into their union (_internal_flatten_bf :4305)
         elif proc == "porosity":   # an array of selections is flattened into their union (:5888-5891); within() is not lowered here
             if self._has_within_before_comma(): raise ScriptError("porosity() of a dynamic selection is not lowered")
@@ -349,8 +350,14 @@ class _Parser:
         self.expect("ch", ")")
         if self.peek() == ("id", "in"):   # `expr in contexts` (evaluate_context md_script.c:3418): one value per context
             self.next(); begs, ends = self.contexts()
+            if proc == "rmsd":   # one fit per context of the atoms of (selection AND context)
+                if ctx_relative: raise ScriptError("a context-relative argument of rmsd() inside `in` contexts is lowered by the md_script shim only")
+                sel = np.asarray(p.idx[0], np.int64)
+                p = api.rmsd(ident, [sel[(sel >= b) & (sel < e)].astype(np.int32) for b, e in zip(begs, ends)])
+                self.expect("ch", ";")
+                return p
             if proc not in ("distance", "angle", "dihedral") or any(m[0] == "other" for m in self.arg_meta) or len(self.arg_meta) != len(p.idx):
-                raise ScriptError("`in` is lowered for distance / angle / dihedral with integer or selection arguments")
+                raise ScriptError("`in` is lowered for distance / angle / dihedral with integer or selection arguments, and for rmsd")
             args = []
             for m in self.arg_meta:
                 if m[0] == "int":   # remap_index_to_context rejects indices outside the context (md_script_functions.inl:1023-1040)
