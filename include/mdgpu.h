@@ -114,6 +114,7 @@ typedef enum mdgpu_op {
     MDGPU_OP_BACKBONE_ANGLES = 20, /* (phi, psi) of every backbone segment per frame -> temporal [F, 2 * n_segments]: VIAMD's "Backbone Operations" pass
                                     * (src/viamd.cpp:488-520 -> md_util_backbone_angles_compute md_util.c:2572-2620) */
     MDGPU_OP_POROSITY = 22,  /* porosity(selection): unoccupied fraction of a voxel grid over the selection's van der Waals spheres -> temporal [F, 1] :5858-6003 */
+    MDGPU_OP_EXPRESSION = 23, /* arithmetic and math functions over other temporal properties of the plan -> temporal [F, dim]: see mdgpu_expr_t :505-603 */
 } mdgpu_op;
 
 /* One property = one `ident = proc(args);` statement whose selections were evaluated statically at compile time
@@ -274,6 +275,46 @@ typedef struct mdgpu_range_arg_t {
  * dynamic selection. mdgpu_plan_create(...) is this function with no ranges. */
 mdgpu_plan* mdgpu_plan_create_with_ranges(const mdgpu_system_desc_t* sys, const mdgpu_property_desc_t* props, size_t num_props,
                                           size_t num_frames, const mdgpu_plan_options_t* opts, const mdgpu_range_arg_t* ranges, size_t num_ranges);
+
+/* A temporal expression: the value of an MDGPU_OP_EXPRESSION property, evaluated per frame on the device after the procedure properties of the
+ * frame (operators md_script_functions.inl:505-571, functions :576-603). The program is postfix: CONST pushes `value`, PROP pushes the row of
+ * property `prop` (a temporal of the plan, not the expression itself), every other node pops its operands and pushes its result. A value is a
+ * float or an array of n floats; `+ - * /` take two floats, an array and a float (either order) or two arrays of equal length, element-wise;
+ * NEG, ABS, FLOOR and CEIL take a float or an array; every other function takes floats only (the reference registers no array form of it).
+ * The property is [F, n] (n = 1 for a float result) with the per-frame aggregates of a multi-valued temporal.
+ * Numerical contract: + - * / NEG ABS FLOOR CEIL MIN MAX SQRT are IEEE float32 operations (MIN / MAX as fminf / fmaxf), bit-equal to the
+ * reference's; the other functions are evaluated in double and rounded to float once (the reference calls glibc's float functions; the two
+ * differ by at most 1 ulp on the reference data, DESIGN.md section 3).
+ * The reference applies `scalar op array` as `array op scalar` (its FLAG_SYMMETRIC_ARGS swaps the operands: `2 - a` is a - 2); a host lowering
+ * from the reference's syntax tree sees the operands already swapped. */
+enum {
+    MDGPU_EXPR_CONST = 0, MDGPU_EXPR_PROP = 1,
+    MDGPU_EXPR_NEG = 2, MDGPU_EXPR_ADD = 3, MDGPU_EXPR_SUB = 4, MDGPU_EXPR_MUL = 5, MDGPU_EXPR_DIV = 6,
+    MDGPU_EXPR_SQRT = 7, MDGPU_EXPR_CBRT = 8, MDGPU_EXPR_ABS = 9, MDGPU_EXPR_FLOOR = 10, MDGPU_EXPR_CEIL = 11, MDGPU_EXPR_COS = 12,
+    MDGPU_EXPR_SIN = 13, MDGPU_EXPR_ASIN = 14, MDGPU_EXPR_ACOS = 15, MDGPU_EXPR_ATAN = 16, MDGPU_EXPR_LOG = 17, MDGPU_EXPR_EXP = 18,
+    MDGPU_EXPR_LOG2 = 19, MDGPU_EXPR_EXP2 = 20, MDGPU_EXPR_LOG10 = 21,
+    MDGPU_EXPR_ATAN2 = 22, MDGPU_EXPR_POW = 23, MDGPU_EXPR_MIN = 24, MDGPU_EXPR_MAX = 25,   /* two operands: atan(y, x) = atan2(y, x) */
+};
+#define MDGPU_EXPR_MAX_DEPTH 16   /* operand stack depth of a program */
+typedef struct mdgpu_expr_node_t {
+    uint32_t kind;                  /* MDGPU_EXPR_* */
+    float value;                    /* CONST */
+    uint32_t prop;                  /* PROP: index into props */
+} mdgpu_expr_node_t;
+typedef struct mdgpu_expr_t {
+    uint32_t prop;                  /* the MDGPU_OP_EXPRESSION property this program computes */
+    const mdgpu_expr_node_t* nodes; /* postfix order */
+    size_t num_nodes;
+} mdgpu_expr_t;
+/* mdgpu_plan_create_with_ranges with temporal expressions beside the descriptors (their layout stays that of earlier hosts). Fails with
+ * MDGPU_ERR_INVALID_ARG for: an EXPRESSION property without exactly one program or a program naming a property that is not an EXPRESSION;
+ * a PROP that names no property, a non-temporal one or the expression itself; expressions that depend on each other in a cycle; a program
+ * that pops an empty stack, holds more than MDGPU_EXPR_MAX_DEPTH operands or does not end with exactly one; two arrays of different lengths;
+ * an array given to a function that takes floats only; an unknown kind. Expressions of expressions are evaluated in dependency order.
+ * mdgpu_plan_create_with_ranges(...) is this function with no expressions. */
+mdgpu_plan* mdgpu_plan_create_ex(const mdgpu_system_desc_t* sys, const mdgpu_property_desc_t* props, size_t num_props, size_t num_frames,
+                                 const mdgpu_plan_options_t* opts, const mdgpu_range_arg_t* ranges, size_t num_ranges,
+                                 const mdgpu_expr_t* exprs, size_t num_exprs);
 void mdgpu_plan_destroy(mdgpu_plan* plan);
 
 /* Frame 0 of the trajectory ("initial configuration", md_script.c:5808): reference structure of sdf() and rmsd(), reference cell of density_*(). */

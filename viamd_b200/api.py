@@ -25,6 +25,11 @@ DIST_BINS = 1024
 VOL_DIM = 128
 
 OP_RDF, OP_SDF, OP_DENSITY_X, OP_DENSITY_Y, OP_DENSITY_Z, OP_DISTANCE, OP_ANGLE, OP_DIHEDRAL, OP_DISTANCE_MIN, OP_DISTANCE_MAX, OP_RMSD, OP_DISTANCE_PAIR, OP_COM, OP_PLANE, OP_WITHIN_COUNT, OP_SHAPE_WEIGHTS, OP_COORD_X, OP_COORD_Y, OP_COORD_Z, OP_BACKBONE_ANGLES, OP_CONTACT_COUNT, OP_POROSITY = 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16, 17, 18, 19, 20, 21, 22
+OP_EXPRESSION = 23
+# node kinds of a temporal expression's postfix program (MDGPU_EXPR_*): operands, then operators and functions
+EXPR_KINDS = {k: i for i, k in enumerate(("const", "prop", "neg", "add", "sub", "mul", "div", "sqrt", "cbrt", "abs", "floor", "ceil", "cos", "sin", "asin",
+                                          "acos", "atan", "log", "exp", "log2", "exp2", "log10", "atan2", "pow", "min", "max"))}
+EXPR_MAX_DEPTH = 16
 CELL_ORTHO, CELL_TRICLINIC, CELL_PBC_X, CELL_PBC_Y, CELL_PBC_Z, CELL_PBC_ALL = 1, 2, 4, 8, 16, 28
 
 
@@ -73,6 +78,14 @@ class _DynArg(C.Structure):   # mdgpu_dynamic_arg_t
 
 class _RangeArg(C.Structure):   # mdgpu_range_arg_t
     _fields_ = [("prop", C.c_uint32), ("arg", C.c_uint32), ("lo", C.c_float * 3), ("hi", C.c_float * 3)]
+
+
+class _ExprNode(C.Structure):   # mdgpu_expr_node_t
+    _fields_ = [("kind", C.c_uint32), ("value", C.c_float), ("prop", C.c_uint32)]
+
+
+class _Expr(C.Structure):   # mdgpu_expr_t
+    _fields_ = [("prop", C.c_uint32), ("nodes", C.POINTER(_ExprNode)), ("num_nodes", C.c_size_t)]
 
 
 class _PropertyDesc(C.Structure):
@@ -136,6 +149,9 @@ def lib() -> C.CDLL:
         L.mdgpu_plan_create_with_ranges.restype = C.c_void_p
         L.mdgpu_plan_create_with_ranges.argtypes = [C.POINTER(_SystemDesc), C.POINTER(_PropertyDesc), C.c_size_t, C.c_size_t, C.POINTER(_PlanOptions),
                                                     C.POINTER(_RangeArg), C.c_size_t]
+        L.mdgpu_plan_create_ex.restype = C.c_void_p
+        L.mdgpu_plan_create_ex.argtypes = [C.POINTER(_SystemDesc), C.POINTER(_PropertyDesc), C.c_size_t, C.c_size_t, C.POINTER(_PlanOptions),
+                                           C.POINTER(_RangeArg), C.c_size_t, C.POINTER(_Expr), C.c_size_t]
         L.mdgpu_plan_destroy.argtypes = [C.c_void_p]
         L.mdgpu_plan_destroy.restype = None
         L.mdgpu_plan_clear.argtypes = [C.c_void_p]
@@ -235,6 +251,7 @@ class Property:
     dyn: dict = field(default_factory=dict)           # {k: (radius_min, radius_max, and_idx | None)}: argument k is within([min:]max, idx[k]) [and and_idx], per frame
     arg_offsets: dict = field(default_factory=dict)   # {k: CSR offsets}: argument k of distance / angle / dihedral / com is an ARRAY of selections (centre of their centres)
     ranges: dict = field(default_factory=dict)        # {k: Range}: argument k is a coordinate range within_x / _y / _z / _xyz(...) [and static], per frame
+    program: Optional[list] = None                    # OP_EXPRESSION: the postfix program, see expression()
 
 
 class Within:
@@ -497,6 +514,18 @@ def rmsd(name, idx):
     return Property(name, OP_RMSD, [np.asarray(idx, np.int32)])
 
 
+def expression(name, program):
+    """A temporal expression: arithmetic and math functions over other temporal properties of the plan, evaluated per frame on the device
+    (operators md_script_functions.inl:505-571, functions :576-603; MDGPU_OP_EXPRESSION). `program` is postfix, a list of nodes:
+    ("const", value) | ("prop", name or index of a temporal property of the same plan) | (kind,) for kind in EXPR_KINDS — "neg", "add", "sub",
+    "mul", "div" and the functions. Element-wise on arrays as the reference: see include/mdgpu.h (mdgpu_expr_t) for the rules."""
+    prog = []
+    for n in program:
+        if n[0] not in EXPR_KINDS: raise ValueError(f"unknown expression node {n!r}")
+        prog.append((n[0], float(n[1]) if n[0] == "const" else 0.0, n[1] if n[0] == "prop" else None))
+    return Property(name, OP_EXPRESSION, program=prog)
+
+
 def porosity(name, idx):
     """porosity(selection): per frame, the unoccupied fraction of a bit grid (longest axis 512 voxels) over the bounding box of the selection's van
     der Waals spheres (_porosity md_script_functions.inl:5858). Needs System.radius. 0 for a triclinic cell or an empty selection."""
@@ -644,11 +673,22 @@ class Plan:
         if devices:
             o.num_devices = len(devices)
             for g, dv in enumerate(devices): o.devices[g] = int(dv)
-        if ranges:
-            rarr = (_RangeArg * len(ranges))()
-            for j, (i, k, r) in enumerate(ranges):
-                rarr[j].prop = i; rarr[j].arg = k
-                for c in range(3): rarr[j].lo[c] = float(r.lo[c]); rarr[j].hi[c] = float(r.hi[c])
+        rarr = (_RangeArg * len(ranges))()
+        for j, (i, k, r) in enumerate(ranges):
+            rarr[j].prop = i; rarr[j].arg = k
+            for c in range(3): rarr[j].lo[c] = float(r.lo[c]); rarr[j].hi[c] = float(r.hi[c])
+        exprs = [(i, p.program) for i, p in enumerate(self.properties) if p.program is not None]
+        if exprs:   # beside the descriptors: mdgpu_expr_t, operands named by property index
+            index = {p.name: i for i, p in enumerate(self.properties)}
+            earr = (_Expr * len(exprs))()
+            for j, (i, prog) in enumerate(exprs):
+                nodes = (_ExprNode * len(prog))(); self._keep.append(nodes)
+                for m, (kind, value, ref) in enumerate(prog):
+                    nodes[m].kind = EXPR_KINDS[kind]; nodes[m].value = value
+                    if kind == "prop": nodes[m].prop = index[ref] if isinstance(ref, str) else int(ref)
+                earr[j].prop = i; earr[j].nodes = nodes; earr[j].num_nodes = len(prog)
+            self._h = L.mdgpu_plan_create_ex(C.byref(sd), descs, len(self.properties), self.num_frames, C.byref(o), rarr, len(ranges), earr, len(exprs))
+        elif ranges:
             self._h = L.mdgpu_plan_create_with_ranges(C.byref(sd), descs, len(self.properties), self.num_frames, C.byref(o), rarr, len(ranges))
         else:
             self._h = L.mdgpu_plan_create(C.byref(sd), descs, len(self.properties), self.num_frames, C.byref(o))

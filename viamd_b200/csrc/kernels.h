@@ -1,4 +1,4 @@
-// kernels.h — host-callable launchers of the per-batch kernels (defined in cells.cu, rdf.cu, sdf.cu, props.cu, porosity.cu, synth.cu)
+// kernels.h — host-callable launchers of the per-batch kernels (defined in cells.cu, rdf.cu, sdf.cu, props.cu, porosity.cu, expr.cu, synth.cu)
 #pragma once
 #include "common.cuh"
 
@@ -166,6 +166,11 @@ void launch_coord_rows(const BatchFrames& fr, const int32_t* d_idx, uint32_t n, 
 void launch_temporal_histogram(const float* d_values, const unsigned long long* d_mask, uint32_t num_frames, uint32_t dim, float range_min, float range_max, float inv_range,
                                uint32_t num_bins, int aggregate, uint32_t* d_counts, uint32_t* d_totals, cudaStream_t s);
 void launch_mean_u32(const uint32_t* d_in, float* d_out, size_t count, unsigned long long n, cudaStream_t s);
+
+// expr.cu — temporal expressions (MDGPU_OP_EXPRESSION): one launch per dependency level of a batch, one block row per expression
+struct ExprNode { uint32_t kind; float value; const float* src; uint32_t src_len; };   // PROP: src = [num_frames][src_len] rows of the operand
+struct ExprProg { uint32_t first_node, num_nodes; float* out; uint32_t len; };         // out = [num_frames][len] rows of the expression
+void launch_temporal_expr(const ExprProg* d_progs, uint32_t n_progs, const ExprNode* d_nodes, uint32_t max_len, uint32_t frame0, int B, cudaStream_t s);
 
 // rama.cu — VIAMD's Ramachandran density maps from the (phi, psi) rows of a backbone-angles temporal
 struct RamaArgs {

@@ -284,6 +284,9 @@ struct mdgpu_plan {
     std::atomic<bool> dirty{true};   // device accumulators changed since the last fold into the host-visible property data
     std::atomic<uint64_t> frames_retired{0};   // frame evaluations of retired batches: the divisor of the running means
     mdg::MultiDevice* multi = nullptr;   // frame blocks on several GPUs from this one process (mdgpu_plan_options_t.num_devices > 1)
+    // temporal expressions: their programs in one buffer, ordered by dependency level; level l is d_expr_progs[expr_level[l] .. expr_level[l+1]),
+    // whose longest row has expr_level_len[l] values
+    DevBuf<ExprNode> d_expr_nodes; DevBuf<ExprProg> d_expr_progs; std::vector<uint32_t> expr_level, expr_level_len;
 };
 
 // get_spatial_acc (md_script_functions.inl:734-760): the system-wide grid of within() has cells of ceil(radius / 6) * 6
@@ -313,11 +316,16 @@ static void build_unwrap_pairs(std::vector<int2>& out, size_t count, const std::
     }
 }
 
+// MIN / MAX of the reference (core/md_common.h:130-134): the second operand unless the first compares below / above it, so a NaN is taken
+// (and dropped again by the next comparison)
+static inline float ref_min(float a, float b) { return a < b ? a : b; }
+static inline float ref_max(float a, float b) { return a > b ? a : b; }
+
 // compute_min_max_mean_variance (md_script.c:5646-5677): min, max, mean and population variance of one frame's values, two passes in float
 static void fold_frame_values(const float* v, size_t len, float& mn, float& mx, float& mean, float& var) {
     const float N = (float)len;
     mn = FLT_MAX; mx = -FLT_MAX; float s1 = 0.0f, s2 = 0.0f;
-    for (size_t i = 0; i < len; ++i) { s1 += v[i]; mn = std::min(mn, v[i]); mx = std::max(mx, v[i]); }
+    for (size_t i = 0; i < len; ++i) { s1 += v[i]; mn = ref_min(mn, v[i]); mx = ref_max(mx, v[i]); }
     s1 = s1 / N;
     for (size_t i = 0; i < len; ++i) s2 += (v[i] - s1) * (v[i] - s1);
     s2 = s2 / N;
@@ -421,12 +429,97 @@ uint64_t mdgpu_launch_count(bool reset) { return reset ? g_launches.exchange(0) 
 
 mdgpu_plan* mdgpu_plan_create(const mdgpu_system_desc_t* sys, const mdgpu_property_desc_t* props, size_t num_props, size_t num_frames,
                               const mdgpu_plan_options_t* opts) {
-    return mdgpu_plan_create_with_ranges(sys, props, num_props, num_frames, opts, nullptr, 0);
+    return mdgpu_plan_create_ex(sys, props, num_props, num_frames, opts, nullptr, 0, nullptr, 0);
 }
 
 mdgpu_plan* mdgpu_plan_create_with_ranges(const mdgpu_system_desc_t* sys, const mdgpu_property_desc_t* props, size_t num_props, size_t num_frames,
                                           const mdgpu_plan_options_t* opts, const mdgpu_range_arg_t* ranges, size_t num_ranges) {
-    if (!sys || !props || !num_props || !num_frames || !sys->num_atoms || (num_ranges && !ranges)) { fail(MDGPU_ERR_INVALID_ARG, "mdgpu_plan_create: invalid arguments"); return nullptr; }
+    return mdgpu_plan_create_ex(sys, props, num_props, num_frames, opts, ranges, num_ranges, nullptr, 0);
+}
+
+}  // extern "C"
+
+// The programs of the temporal expressions of a plan whose other properties are set up: checked (see mdgpu_plan_create_ex), each expression's
+// values per frame from its operands, then the programs in dependency levels -> p->d_expr_*. "" or the error message (an invalid argument).
+static std::string take_expressions(mdgpu_plan* p, const mdgpu_property_desc_t* props, size_t num_props, const mdgpu_expr_t* exprs, size_t num_exprs, cudaError_t& e) {
+    std::vector<const mdgpu_expr_t*> prog(num_props, nullptr);
+    for (size_t j = 0; j < num_exprs; ++j) {
+        const mdgpu_expr_t& x = exprs[j];
+        if (x.prop >= num_props || props[x.prop].op != MDGPU_OP_EXPRESSION) return "expression " + std::to_string(j) + ": property " + std::to_string(x.prop) + " is not an expression property";
+        if (prog[x.prop]) return "property '" + p->props[x.prop].name + "' has more than one program";
+        if (!x.num_nodes || !x.nodes) return "property '" + p->props[x.prop].name + "': empty program";
+        prog[x.prop] = &x;
+    }
+    for (size_t i = 0; i < num_props; ++i) if (props[i].op == MDGPU_OP_EXPRESSION && !prog[i]) return "property '" + p->props[i].name + "' has no program";
+    // operands first: depth-first over the expression operands, in topological order; 1 = on the current path (a cycle), 2 = placed
+    std::vector<int> state(num_props, 0), level(num_props, 0); std::vector<uint32_t> order;
+    std::string er;
+    std::function<bool(uint32_t)> visit = [&](uint32_t i) -> bool {
+        if (state[i] == 2) return true;
+        if (state[i] == 1) { er = "expressions depend on each other in a cycle (through '" + p->props[i].name + "')"; return false; }
+        state[i] = 1;
+        const mdgpu_expr_t& x = *prog[i];
+        for (size_t k = 0; k < x.num_nodes; ++k) {
+            const mdgpu_expr_node_t& n = x.nodes[k];
+            if (n.kind > MDGPU_EXPR_MAX) { er = "'" + p->props[i].name + "': unknown expression node kind " + std::to_string(n.kind); return false; }
+            if (n.kind != MDGPU_EXPR_PROP) continue;
+            if (n.prop >= num_props) { er = "'" + p->props[i].name + "': operand property " + std::to_string(n.prop) + " out of range"; return false; }
+            if (n.prop == i) { er = "'" + p->props[i].name + "': an expression cannot name itself"; return false; }
+            if (props[n.prop].op == MDGPU_OP_EXPRESSION) { if (!visit(n.prop)) return false; level[i] = std::max(level[i], level[n.prop] + 1); }
+            else if (!p->props[n.prop].d_temporal.get()) { er = "'" + p->props[i].name + "': operand '" + p->props[n.prop].name + "' is not a temporal property"; return false; }
+        }
+        state[i] = 2; order.push_back(i);
+        return true;
+    };
+    for (size_t i = 0; i < num_props; ++i) if (prog[i] && !visit((uint32_t)i)) return er;
+    // value counts: a float is 0 on the stack of counts, an array its length (a temporal of one value per frame is a float)
+    for (uint32_t i : order) {
+        const mdgpu_expr_t& x = *prog[i]; const std::string who = "'" + p->props[i].name + "': ";
+        std::vector<size_t> st;
+        for (size_t k = 0; k < x.num_nodes; ++k) {
+            const uint32_t kind = x.nodes[k].kind;
+            if (kind == MDGPU_EXPR_CONST || kind == MDGPU_EXPR_PROP) {
+                if (st.size() == MDGPU_EXPR_MAX_DEPTH) return who + "more than " + std::to_string(MDGPU_EXPR_MAX_DEPTH) + " operands on the stack";
+                const size_t len = kind == MDGPU_EXPR_CONST ? 1 : p->props[x.nodes[k].prop].len;
+                st.push_back(len > 1 ? len : 0);
+                continue;
+            }
+            const bool binary = kind >= MDGPU_EXPR_ATAN2 || (kind >= MDGPU_EXPR_ADD && kind <= MDGPU_EXPR_DIV);
+            if (st.size() < (binary ? 2u : 1u)) return who + "the program pops an empty stack";
+            const bool elementwise = binary ? kind <= MDGPU_EXPR_DIV : (kind == MDGPU_EXPR_NEG || kind == MDGPU_EXPR_ABS || kind == MDGPU_EXPR_FLOOR || kind == MDGPU_EXPR_CEIL);
+            const size_t b = st.back(), a = binary ? st[st.size() - 2] : 0;
+            if (!elementwise && (a || b)) return who + "an array given to a function that takes floats only";
+            if (a && b && a != b) return who + "arrays of different lengths (" + std::to_string(a) + " and " + std::to_string(b) + ")";
+            if (binary) st.pop_back();
+            st.back() = std::max(a, b);
+        }
+        if (st.size() != 1) return who + "the program leaves " + std::to_string(st.size()) + " values instead of one";
+        if ((e = set_temporal(p->props[i], p->num_frames, st[0] ? st[0] : 1)) != cudaSuccess) return "";
+    }
+    std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return level[a] < level[b]; });
+    std::vector<ExprNode> nodes; std::vector<ExprProg> progs;
+    for (uint32_t i : order) {
+        const mdgpu_expr_t& x = *prog[i];
+        if (p->expr_level.size() <= (size_t)level[i]) { p->expr_level.push_back((uint32_t)progs.size()); p->expr_level_len.push_back(0); }
+        p->expr_level_len[level[i]] = std::max(p->expr_level_len[level[i]], (uint32_t)p->props[i].len);
+        progs.push_back(ExprProg{ (uint32_t)nodes.size(), (uint32_t)x.num_nodes, p->props[i].d_temporal.get(), (uint32_t)p->props[i].len });
+        for (size_t k = 0; k < x.num_nodes; ++k) {
+            const mdgpu_expr_node_t& n = x.nodes[k];
+            const Prop* src = n.kind == MDGPU_EXPR_PROP ? &p->props[n.prop] : nullptr;
+            nodes.push_back(ExprNode{ n.kind, n.value, src ? src->d_temporal.get() : nullptr, src ? (uint32_t)src->len : 0u });
+        }
+    }
+    p->expr_level.push_back((uint32_t)progs.size());
+    if ((e = p->d_expr_nodes.upload(nodes.data(), nodes.size())) != cudaSuccess) return "";
+    e = p->d_expr_progs.upload(progs.data(), progs.size());
+    return "";
+}
+
+extern "C" {
+
+mdgpu_plan* mdgpu_plan_create_ex(const mdgpu_system_desc_t* sys, const mdgpu_property_desc_t* props, size_t num_props, size_t num_frames,
+                                 const mdgpu_plan_options_t* opts, const mdgpu_range_arg_t* ranges, size_t num_ranges, const mdgpu_expr_t* exprs, size_t num_exprs) {
+    if (!sys || !props || !num_props || !num_frames || !sys->num_atoms || (num_ranges && !ranges) || (num_exprs && !exprs)) { fail(MDGPU_ERR_INVALID_ARG, "mdgpu_plan_create: invalid arguments"); return nullptr; }
     // the coordinate range of each (property, argument), if any
     std::vector<std::array<const mdgpu_range_arg_t*, 4>> range_of(num_props, std::array<const mdgpu_range_arg_t*, 4>{});
     for (size_t r = 0; r < num_ranges; ++r) {
@@ -446,12 +539,12 @@ mdgpu_plan* mdgpu_plan_create_with_ranges(const mdgpu_system_desc_t* sys, const 
             if (!getenv("MDGPU_ALLOW_DUPLICATE_DEVICES")) for (uint32_t h = 0; h < g; ++h) if (o.devices[h] == o.devices[g]) { fail(MDGPU_ERR_INVALID_ARG, "device %d listed twice", o.devices[g]); return nullptr; }
         }
         mdgpu_plan_options_t one = o; one.num_devices = 0; one.device = o.devices[0];
-        mdgpu_plan* root = mdgpu_plan_create_with_ranges(sys, props, num_props, num_frames, &one, ranges, num_ranges);
+        mdgpu_plan* root = mdgpu_plan_create_ex(sys, props, num_props, num_frames, &one, ranges, num_ranges, exprs, num_exprs);
         if (!root) return nullptr;
         root->multi = new MultiDevice(); root->multi->devices.assign(o.devices, o.devices + o.num_devices);
         for (uint32_t g = 1; g < o.num_devices; ++g) {
             one.device = o.devices[g];
-            mdgpu_plan* q = mdgpu_plan_create_with_ranges(sys, props, num_props, num_frames, &one, ranges, num_ranges);
+            mdgpu_plan* q = mdgpu_plan_create_ex(sys, props, num_props, num_frames, &one, ranges, num_ranges, exprs, num_exprs);
             if (!q) { destroy_plan(root); return nullptr; }
             root->multi->peers.push_back(q);
         }
@@ -758,6 +851,8 @@ mdgpu_plan* mdgpu_plan_create_with_ranges(const mdgpu_system_desc_t* sys, const 
             if (e == cudaSuccess) e = pr.d_soff.upload(pr.h_soff.data(), pr.h_soff.size());
             if (e == cudaSuccess) e = set_temporal(pr, num_frames, pr.n_struct);
             break; }
+        case MDGPU_OP_EXPRESSION:   // its values per frame follow from its program's operands: take_expressions, once every property is set up
+            continue;
         default:
             return bail(MDGPU_ERR_UNSUPPORTED, "property '" + pr.name + "': unsupported operation " + std::to_string(pr.op));
         }
@@ -765,6 +860,16 @@ mdgpu_plan* mdgpu_plan_create_with_ranges(const mdgpu_system_desc_t* sys, const 
         pr.vptr = pr.values.data(); pr.amean = pr.agg_mean.data(); pr.avar = pr.agg_var.data(); pr.aext = pr.agg_ext.data();
         pr.data.num_values = pr.values.size(); pr.data.values = pr.vptr;
         pr.data.weights = pr.is_dist() ? pr.vptr + MDGPU_DIST_BINS : nullptr;
+    }
+    {
+        cudaError_t e = cudaSuccess;
+        const std::string er = take_expressions(p, props, num_props, exprs, num_exprs, e);
+        if (!er.empty()) return bail(MDGPU_ERR_INVALID_ARG, er);
+        if (e != cudaSuccess) return bail(MDGPU_ERR_CUDA, std::string("device allocation failed: ") + cudaGetErrorString(e));
+        for (auto& pr : p->props) if (pr.op == MDGPU_OP_EXPRESSION) {
+            pr.vptr = pr.values.data(); pr.amean = pr.agg_mean.data(); pr.avar = pr.agg_var.data(); pr.aext = pr.agg_ext.data();
+            pr.data.num_values = pr.values.size(); pr.data.values = pr.vptr;
+        }
     }
     for (size_t i = 0; i < num_props; ++i) for (size_t j = 0; j < i; ++j) {
         Prop& a = p->props[i]; Prop& b = p->props[j];
@@ -1242,6 +1347,8 @@ static int enqueue_batch(mdgpu_plan* p, Slot& s, const BatchFrames& fr, uint32_t
         }
         pr.frames_accumulated += (uint64_t)B;
     }
+    for (size_t l = 0; l + 1 < p->expr_level.size(); ++l)   // temporal expressions, after the rows they read: level by level, on the batch's stream
+        launch_temporal_expr(p->d_expr_progs.get() + p->expr_level[l], p->expr_level[l + 1] - p->expr_level[l], p->d_expr_nodes.get(), p->expr_level_len[l], frame0, B, s.stream);
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaMemcpyAsync(s.h_err.get(), s.d_err.get(), sizeof(int), cudaMemcpyDeviceToHost, s.stream));   // read when the slot is retired
     CUDA_TRY(cudaEventRecord(s.done, s.stream));
@@ -1765,7 +1872,7 @@ static double sphere_volume(double r) { return (4.0 / 3.0) * 3.1415926535897932 
 static void fold_temporal_rows(Prop& pr, uint32_t f, bool reset) {
     if (reset) { pr.data.min_value = +FLT_MAX; pr.data.max_value = -FLT_MAX; }
     float mn, mx, s1, s2; fold_frame_values(pr.vptr + (size_t)f * pr.len, pr.len, mn, mx, s1, s2);
-    pr.data.min_value = std::min(pr.data.min_value, mn); pr.data.max_value = std::max(pr.data.max_value, mx);
+    pr.data.min_value = ref_min(pr.data.min_value, mn); pr.data.max_value = ref_max(pr.data.max_value, mx);   // md_script.c:5885-5886
     if (pr.len > 1) { pr.amean[f] = s1; pr.avar[f] = s2; pr.aext[2 * f] = mn; pr.aext[2 * f + 1] = mx; }
 }
 static void temporal_ranges(Prop& pr) {

@@ -9,6 +9,8 @@ Supported statements:  ident = proc(args);   with proc in
     rdf(sel, sel, cutoff | min:max)   sdf(residue(a:b) | sel-array, sel, cutoff)   density_x|_y|_z(sel)
     distance(i, j)   angle(i, j, k)   dihedral(i, j, k, l)            (1-based atom indices as in md_script)
     porosity(sel)                                                        (needs System.radius)
+and temporal expressions: + - * / and unary -, the functions sqrt cbrt abs floor ceil cos sin asin acos atan log exp log2 exp2 log10
+atan(y, x) atan2 pow min max, over numbers, PI / TAU / E, earlier temporal properties and inline calls of the procedures above.
 Selections (evaluated once, statically, to ascending atom index lists — md_script.c:5492-5524):
     all | element('O') | name('C2*') | resname('SOL') | atom(a:b) | residue(a:b) | `and` / `or` / `not` of these
 Dynamic selections (evaluated per frame on the device), alone or `static and ...` in either order, where a consumer accepts them:
@@ -283,9 +285,93 @@ class _Parser:
             elif t[0] == "id" and t[1] in names: return True
         return False
 
+    def _is_call_statement(self) -> bool:
+        """does the right-hand side that starts here consist of one procedure call (optionally `in` contexts)"""
+        if self.peek()[0] != "id" or self.peek()[1] in _FUNCS or self.i + 1 >= len(self.t) or self.t[self.i + 1] != ("ch", "("): return False
+        depth = 0
+        for j in range(self.i + 1, len(self.t)):
+            if self.t[j] == ("ch", "("): depth += 1
+            elif self.t[j] == ("ch", ")"):
+                depth -= 1
+                if depth == 0: return j + 1 < len(self.t) and self.t[j + 1] in (("ch", ";"), ("id", "in"))
+        return False
+
     def statement(self) -> api.Property:
         ident = self.expect("id")[1]; self.expect("ch", "=")
+        if not self._is_call_statement(): return self.expression(ident)
         proc = self.expect("id")[1]; self.expect("ch", "(")
+        return self.call(ident, proc)
+
+    # ---- temporal expressions: the reference's tree (parse_arithmetic / fix_precedence, md_script.c:2314, :1196), then its operand order
+    def expression(self, ident) -> api.Property:
+        self.calls, self.ident = 0, ident
+        tree = self._expr()
+        if self.peek() == ("id", "in"): raise ScriptError("an expression inside `in` contexts is not lowered")
+        self.expect("ch", ";")
+        prog, n = self._emit(tree)
+        p = api.expression(ident, prog); p.values_per_frame = max(n, 1)
+        return p
+
+    def _expr(self):
+        """right-recursive as the reference parses: operand [op rest], `-` rest; each new node then goes through fix_precedence"""
+        if self.peek() == ("ch", "-"):
+            self.next(); node = ["neg", self._expr()]
+            c = node[1]
+            if c[0] in _PREC and c[0] != "neg" and _PREC[c[0]] > _PREC["neg"]: node = [c[0], ["neg", c[1]], c[2]]   # the unary branch rotates once
+            return node
+        lhs = self._operand()
+        if self.peek()[0] == "ch" and self.peek()[1] in "+-*/":
+            op = {"+": "add", "-": "sub", "*": "mul", "/": "div"}[self.next()[1]]
+            return _fix([op, lhs, self._expr()])
+        return lhs
+
+    def _operand(self):
+        tok = self.next()
+        if tok == ("ch", "("):
+            e = self._expr(); self.expect("ch", ")"); return ["paren", e]
+        if tok[0] == "num": return ["const", float(np.float32(float(tok[1])))]   # an integer literal is cast to float by the front end
+        if tok[0] != "id": raise ScriptError(f"unexpected token {tok[1]!r} in an expression")
+        name = tok[1]
+        if name in _CONSTANTS: return ["const", _CONSTANTS[name]]
+        if self.peek() != ("ch", "("):
+            if name not in self.known: raise ScriptError(f"'{name}' is not an earlier temporal property of the script")
+            return ["prop", name]
+        if name in _FUNCS:
+            self.next(); args = [self._expr()]
+            while self.peek() == ("ch", ","): self.next(); args.append(self._expr())
+            self.expect("ch", ")")
+            return ["func", name, args]
+        self.next()   # an inline call of a procedure: a hidden property ident#k
+        hidden = f"{self.ident}#{self.calls}"; self.calls += 1
+        p = self.call(hidden, name, inline=True)
+        if p.op in (api.OP_RDF, api.OP_SDF, api.OP_DENSITY_X, api.OP_DENSITY_Y, api.OP_DENSITY_Z): raise ScriptError("arithmetic on distributions and volumes is not lowered")
+        self.hidden.append(p); self.known[hidden] = p
+        return ["prop", hidden]
+
+    def _emit(self, node):
+        """postfix program and value count (0 = float) of a tree, with the reference's typing: `float op array` is applied as `array op float`
+        (FLAG_SYMMETRIC_ARGS swaps the operands, md_script.c:3802); functions other than abs / floor / ceil take floats only"""
+        k = node[0]
+        if k == "paren": return self._emit(node[1])
+        if k == "const": return [("const", node[1])], 0
+        if k == "prop":
+            n = _values_per_frame(self.known[node[1]])
+            return [("prop", node[1])], (n if n > 1 else 0)
+        if k == "neg":
+            p, n = self._emit(node[1]); return p + [("neg",)], n
+        if k == "func":
+            name, args = node[1], node[2]
+            if len(args) not in _FUNCS[name]: raise ScriptError(f"{name}() takes {' or '.join(map(str, _FUNCS[name]))} arguments")
+            parts = [self._emit(a) for a in args]
+            if any(n for _, n in parts) and name not in ("abs", "floor", "ceil"): raise ScriptError(f"{name}() takes floats only")
+            kind = name if len(args) == 1 else {"atan": "atan2"}.get(name, name)
+            return sum((p for p, _ in parts), []) + [(kind,)], max(n for _, n in parts)
+        (pa, na), (pb, nb) = self._emit(node[1]), self._emit(node[2])
+        if na and nb and na != nb: raise ScriptError(f"arrays of different lengths ({na} and {nb})")
+        if nb and not na: pa, pb = pb, pa   # the symmetric match puts the array first
+        return pa + pb + [(k,)], max(na, nb)
+
+    def call(self, ident, proc, inline=False) -> api.Property:
         self.arg_meta = []   # how each argument of distance / angle / dihedral was written (index()): decides its meaning inside `in` contexts
         if proc == "rdf":
             wr = rr = None
@@ -348,6 +434,7 @@ class _Parser:
         else:
             raise ScriptError(f"procedure '{proc}' is outside the GPU hot-path scope")
         self.expect("ch", ")")
+        if inline: return p
         if self.peek() == ("id", "in"):   # `expr in contexts` (evaluate_context md_script.c:3418): one value per context
             self.next(); begs, ends = self.contexts()
             if proc == "rmsd":   # one fit per context of the atoms of (selection AND context)
@@ -391,11 +478,45 @@ class _Parser:
         raise ScriptError(f"unsupported context expression '{f}'")
 
 
+_PREC = {"neg": 2, "mul": 3, "div": 3, "add": 4, "sub": 4}   # operator_precedence (md_script.c:502)
+_FUNCS = {f: (1,) for f in ("sqrt", "cbrt", "abs", "floor", "ceil", "cos", "sin", "asin", "acos", "log", "exp", "log2", "exp2", "log10")}
+_FUNCS.update(atan=(1, 2), atan2=(2,), pow=(2,), min=(2,), max=(2,))
+_CONSTANTS = {"PI": float(np.float32(3.14159265358)), "TAU": float(np.float32(6.28318530718)), "E": float(np.float32(2.71828182845))}   # md_script_functions.inl:456-466
+
+
+def _fix(node):
+    """fix_precedence (md_script.c:1196) on a new binary node whose right child was parsed first: rotate while the right child binds looser or
+    equally (left to right), then fix the new left child"""
+    c = node[2]
+    if c[0] in _PREC and c[0] != "neg" and (_PREC[c[0]] >= _PREC[node[0]]):
+        node = [c[0], [node[0], node[1], c[1]], c[2]]
+        node[1] = _fix(node[1])
+    return node
+
+
+def _values_per_frame(p: api.Property) -> int:
+    """values per frame of a temporal property, 0 for a distribution or volume"""
+    if p.op in (api.OP_RDF, api.OP_SDF, api.OP_DENSITY_X, api.OP_DENSITY_Y, api.OP_DENSITY_Z): return 0
+    if p.op == api.OP_EXPRESSION: return p.values_per_frame
+    if p.op == api.OP_COM: return 3
+    if p.op == api.OP_PLANE: return 4
+    if p.op == api.OP_DISTANCE_PAIR:
+        n = [len(o) - 1 if o is not None else int(np.size(i)) for o, i in ((p.structure_offsets, p.idx[0]), (p.structure_offsets_b, p.idx[1]))]
+        return n[0] * n[1]
+    if p.op in (api.OP_COORD_X, api.OP_COORD_Y, api.OP_COORD_Z): return p.num_structures or int(np.size(p.idx[0]))
+    if p.op in (api.OP_DISTANCE, api.OP_ANGLE, api.OP_DIHEDRAL, api.OP_RMSD, api.OP_CONTACT_COUNT): return max(p.num_structures, 1)
+    return 1
+
+
 def compile_script(src: str, system: api.System) -> List[api.Property]:
-    """`md_script_ir_compile_from_source` stand-in for the supported statement subset."""
+    """`md_script_ir_compile_from_source` stand-in for the supported statement subset. The procedure calls inside temporal expressions become
+    hidden properties (named ident#k) after the script's own, as the md_script shim appends them."""
     ps = _Parser(_tokens(src), system); out = []
+    ps.known, ps.hidden = {}, []
     while ps.peek()[0] != "eof":
-        out.append(ps.statement())
+        p = ps.statement()
+        if _values_per_frame(p): ps.known[p.name] = p
+        out.append(p)
     if not out:
         raise ScriptError("No properties present in ir")
-    return out
+    return out + ps.hidden
