@@ -115,6 +115,8 @@ typedef enum mdgpu_op {
                                     * (src/viamd.cpp:488-520 -> md_util_backbone_angles_compute md_util.c:2572-2620) */
     MDGPU_OP_POROSITY = 22,  /* porosity(selection): unoccupied fraction of a voxel grid over the selection's van der Waals spheres -> temporal [F, 1] :5858-6003 */
     MDGPU_OP_EXPRESSION = 23, /* arithmetic and math functions over other temporal properties of the plan -> temporal [F, dim]: see mdgpu_expr_t :505-603 */
+    MDGPU_OP_SECONDARY_STRUCTURE = 24, /* md_secondary_structure_t of every backbone segment per frame -> temporal [F, n_segments]: the other half of VIAMD's
+                                        * "Backbone Operations" pass (src/viamd.cpp:488-525 -> md_util_backbone_secondary_structure_infer md_util.c:2552) */
 } mdgpu_op;
 
 /* One property = one `ident = proc(args);` statement whose selections were evaluated statically at compile time
@@ -155,6 +157,23 @@ typedef enum mdgpu_op {
  *              (md_protein_backbone_data_t::segment.atoms of the segment and its neighbours), back to back; -1 in any of the five marks a segment without angles (the first / last residue of a chain, chains shorter than 4:
  *              md_util.c:2588-2592) whose two values stay 0. Row f holds md_backbone_angles_t[num_structures] = (phi, psi) pairs in radians:
  *              phi = dihedral(C', N, CA, C), psi = dihedral(N, CA, C, N') with md_util_min_image_vec3 on the bond vectors, as `dihedral` evaluates.
+ *   SECONDARY_STRUCTURE: idx[0] = for each of the num_structures backbone segments its atoms N, CA, C, O, HN back to back
+ *              (md_protein_backbone_data_t::segment.atoms); HN is -1 when the residue has none, and H is then estimated as the reference does
+ *              (estimate_HN from the previous segment's C, estimate_HN_term for the first segment of a range, md_util.c:1974-1989). The backbone
+ *              ranges (chains) travel in structure_offsets_b with num_structures_b = the range count: backbone->range.offset, range.count + 1
+ *              ascending entries from 0 to num_structures. Row f holds the md_secondary_structure_t code (1 coil .. 8 beta bridge) of every segment
+ *              as a float; mdgpu_plan_secondary_structure returns the rows as md_secondary_structure_t. Numerical contract: every float
+ *              operation is the reference's, in its order and rounding, with two exceptions: vec4_rsqrt of the H-bond energy is 1.0f / sqrtf(d2)
+ *              (the reference's rsqrtps + one Newton step depends on the host CPU), and the bend angle's atan2f is CUDA's, which can differ from
+ *              glibc's in the last ulp (the C restatement oracle/md_dssp.c uses glibc's, so the two agree in the bend decisions, not bit for bit in
+ *              the angle); turn masks and flags start at zero (the reference takes them
+ *              from uncleared temporary memory, md_util.c:2071, 2085). The rows equal the reference's wherever no candidate energy lies within
+ *              1e-3 of -0.5, no donor's 2nd and 3rd lowest energies lie within 1e-3 of each other and no bend angle lies within 1e-4 rad of 70
+ *              degrees. Candidate pairs are those of the reference's cell-grid walk over the CA positions at 9 A with the frame's cell
+ *              (md_spatial_acc_for_each_internal_pair_within_cutoff); energies use the raw coordinates. A frame whose grid has fewer than 2n + 1
+ *              cells on a periodic axis (n the neighbour reach; an orthorhombic axis under 27 A), or whose cell is triclinic without periodicity on
+ *              all axes, fails with MDGPU_ERR_UNSUPPORTED: that walk can report a pair twice. mdgpu_plan_create fails with MDGPU_ERR_INVALID_ARG for
+ *              no segments, an atom out of range (only HN may be -1), and range offsets that are missing, not ascending or not from 0 to num_structures.
  *   RMSD     : idx[0] = the atoms of the (flattened) selection; needs the initial frame and, to make molecules whole, the bond connectivity.
  *              With num_structures = n > 0 the statement was `rmsd(x) in <n contexts>` (evaluate_context md_script.c:3418): idx[0] holds n groups
  *              back to back, group c = the atoms of (flattened x AND context c), delimited by structure_offsets[n+1], or `structure_size` atoms each
@@ -407,6 +426,11 @@ int mdgpu_plan_property_histogram(mdgpu_plan* plan, size_t prop, uint32_t num_bi
  * in the reference's order, so the map equals the reference's value for value (only the sign of a zero may differ); out_sum[c] = (float)(double)n. */
 int mdgpu_plan_rama_density(mdgpu_plan* plan, size_t prop, const uint32_t* segments, const uint32_t class_offsets[5], uint32_t frame_beg, uint32_t frame_end,
                             float sigma, float* out_tex, float out_sum[4]);
+
+/* The secondary structure of frames [frame_beg, frame_end) of an MDGPU_OP_SECONDARY_STRUCTURE property: out[(f - frame_beg) * S + i] = the
+ * md_secondary_structure_t of segment i (4 bytes each), ready to be copied into VIAMD's trajectory_data.secondary_structure at stride S per frame.
+ * Frames not evaluated yet hold 0 (MD_SECONDARY_STRUCTURE_UNKNOWN). Implies mdgpu_plan_sync; runs on devices[0] of a multi-device plan. */
+int mdgpu_plan_secondary_structure(mdgpu_plan* plan, size_t prop, uint32_t frame_beg, uint32_t frame_end, int32_t* out);
 
 /* Exact integer results (what parity is asserted on).
  *  _counts: accumulated counts over all evaluated frames: RDF 1024 x u64 bins; SDF 128^3 x u64 voxels (widened from u32);

@@ -26,6 +26,7 @@ VOL_DIM = 128
 
 OP_RDF, OP_SDF, OP_DENSITY_X, OP_DENSITY_Y, OP_DENSITY_Z, OP_DISTANCE, OP_ANGLE, OP_DIHEDRAL, OP_DISTANCE_MIN, OP_DISTANCE_MAX, OP_RMSD, OP_DISTANCE_PAIR, OP_COM, OP_PLANE, OP_WITHIN_COUNT, OP_SHAPE_WEIGHTS, OP_COORD_X, OP_COORD_Y, OP_COORD_Z, OP_BACKBONE_ANGLES, OP_CONTACT_COUNT, OP_POROSITY = 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16, 17, 18, 19, 20, 21, 22
 OP_EXPRESSION = 23
+OP_SECONDARY_STRUCTURE = 24
 # node kinds of a temporal expression's postfix program (MDGPU_EXPR_*): operands, then operators and functions
 EXPR_KINDS = {k: i for i, k in enumerate(("const", "prop", "neg", "add", "sub", "mul", "div", "sqrt", "cbrt", "abs", "floor", "ceil", "cos", "sin", "asin",
                                           "acos", "atan", "log", "exp", "log2", "exp2", "log10", "atan2", "pow", "min", "max"))}
@@ -502,6 +503,16 @@ def backbone_angles(name, five):
     return Property(name, OP_BACKBONE_ANGLES, [five.reshape(-1)], num_structures=len(five))
 
 
+def secondary_structure(name, atoms, range_offsets):
+    """The secondary structure of every backbone segment per frame (MDGPU_OP_SECONDARY_STRUCTURE, md_util_backbone_secondary_structure_infer):
+    `atoms` is [n_segments, 5] = N, CA, C, O, HN of each segment (md_protein_backbone_data_t::segment.atoms; HN -1 when estimated),
+    `range_offsets` the backbone ranges (chains) as range.count + 1 ascending offsets from 0 to n_segments. The property is [F, n_segments]
+    md_secondary_structure_t codes as floats; Plan.secondary_structure returns them as int32."""
+    atoms = np.ascontiguousarray(atoms, np.int32).reshape(-1, 5)
+    return Property(name, OP_SECONDARY_STRUCTURE, [atoms.reshape(-1)], num_structures=len(atoms),
+                    structure_offsets_b=np.ascontiguousarray(range_offsets, np.uint32))
+
+
 def rmsd(name, idx):
     """rmsd(selection): mass-weighted RMSD of the selection's atoms against the initial frame after wrap, bond-walk unwrap and an optimal
     rotation (_rmsd md_script_functions.inl:4287). Needs System.conn_offset / conn_idx to make molecules whole, as the reference does.
@@ -753,6 +764,17 @@ class Plan:
         _check(L.mdgpu_plan_rama_density(self._h, i, seg.ctypes.data if seg.size else None, off.ctypes.data, int(frame_beg), end, float(sigma),
                                           tex.ctypes.data, sums.ctypes.data))
         return tex, sums
+
+    def secondary_structure(self, name, frame_beg: int = 0, frame_end: Optional[int] = None):
+        """The rows of secondary-structure property `name` for frames [frame_beg, frame_end) as int32 md_secondary_structure_t [frames, n_segments]
+        (mdgpu_plan_secondary_structure); frames not evaluated yet are 0 (unknown)."""
+        i = self._index(name)
+        end = self.num_frames if frame_end is None else int(frame_end)
+        S = int(self.properties[i].num_structures)   # the segment count the property was built with
+        out = np.zeros((max(end - int(frame_beg), 0), S), np.int32)
+        L = lib(); L.mdgpu_plan_secondary_structure.argtypes = [C.c_void_p, C.c_size_t, C.c_uint32, C.c_uint32, C.c_void_p]
+        _check(L.mdgpu_plan_secondary_structure(self._h, i, int(frame_beg), end, out.ctypes.data if out.size else None))
+        return out
 
     def exchange_stats(self):
         ms = C.c_double(); n = C.c_uint64(); _check(lib().mdgpu_plan_exchange_stats(self._h, C.byref(ms), C.byref(n))); return ms.value, int(n.value)

@@ -9,7 +9,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libmdgpu.so")
 STAMP = os.path.join(HERE, "build", "flags.txt")   # the flags libmdgpu.so was built with
-SOURCES = ["cells.cu", "rdf.cu", "sdf.cu", "props.cu", "within.cu", "synth.cu", "xtc.cu", "rama.cu", "porosity.cu", "expr.cu", "plan.cu"]
+SOURCES = ["cells.cu", "rdf.cu", "sdf.cu", "props.cu", "within.cu", "synth.cu", "xtc.cu", "rama.cu", "porosity.cu", "expr.cu", "dssp.cu", "plan.cu"]
 ARCH = "arch=compute_90a,code=sm_90a"   # H100 (Hopper)
 NVCC_FLAGS = [
     "-gencode", ARCH, "-lineinfo", "-O3", "-std=c++17",

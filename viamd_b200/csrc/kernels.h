@@ -1,4 +1,4 @@
-// kernels.h — host-callable launchers of the per-batch kernels (defined in cells.cu, rdf.cu, sdf.cu, props.cu, porosity.cu, expr.cu, synth.cu)
+// kernels.h — host-callable launchers of the per-batch kernels (defined in cells.cu, rdf.cu, sdf.cu, props.cu, porosity.cu, expr.cu, dssp.cu, synth.cu)
 #pragma once
 #include "common.cuh"
 
@@ -211,6 +211,23 @@ struct PorosityArgs {
     uint32_t frame0;                 // global index of the sub-batch's first frame
 };
 void launch_porosity(const PorosityArgs& a, int nf, cudaStream_t s);
+
+// dssp.cu — secondary structure of every backbone segment per frame (md_util_backbone_secondary_structure_infer)
+constexpr uint32_t SS_RES_FLOATS = 20;   // per (frame, segment): N, CA, C, O, H (xyz each), the CA's cell-grid coordinates (3) and packed cell
+struct SsArgs {
+    BatchFrames frames;
+    const int32_t* atoms;            // [S][5] N, CA, C, O, HN (-1: estimated) in the frames' atom space
+    const uint32_t* seg;             // [S][3] range id, range begin, range end of each segment
+    uint32_t S;
+    const FrameGeom* geom;           // [B] the candidate walk's grid (cell extent and cutoff 9 A) of each frame
+    float* res;                      // [B][S][SS_RES_FLOATS] scratch
+    float4* hb;                      // [B][S] per donor: the two lowest energies <= -0.5 (acceptor bits, energy, acceptor bits, energy)
+    uint32_t* bits;                  // [B][2][S] scratch: turn / bend bits, then the structure flags
+    float* out;                      // [num_frames][S] codes as floats
+    uint32_t frame0;
+    int* err;                        // MDGPU_ERR_UNSUPPORTED: a frame's grid cannot visit each candidate pair once
+};
+void launch_secondary_structure(const SsArgs& a, int B, bool tri, cudaStream_t s);
 
 // xtc.cu — compressed trajectory frames expanded on the device
 struct XtcFrameInfo {   // written by k_xtc_scan, one per frame

@@ -155,6 +155,7 @@ struct Prop {
     size_t trg_groups = 0;   // rdf: the target argument was an ARRAY of selections: one centre of mass per selection is the target point (h_goff[1] = their CSR offsets in idx[1])
     size_t backbone_segments = 0;   // MDGPU_OP_BACKBONE_ANGLES (evaluated as 2 dihedrals in context per segment): the segments of its (phi, psi) rows
     DevBuf<unsigned long long> d_frame_n;   // porosity: voxels of each frame's grid (N); d_frame_total holds the occupied ones
+    size_t ss_segments = 0; DevBuf<uint32_t> d_ss_seg;   // MDGPU_OP_SECONDARY_STRUCTURE: segments; per segment its range id, range begin and range end
 
     // The result accumulators, each once: f(&Prop::member) in turn until one returns non-zero. They are zeroed by mdgpu_plan_clear, and
     // multi_sync sums them onto the root device (rows of frames a device did not evaluate are zero there) and zeroes them on the peers.
@@ -187,6 +188,8 @@ struct PropScratch {   // per (stream slot, property)
     mdgpu_unitcell_t nn_cell{}; size_t nn_stride = 0; bool nn_valid = false;   // candidate-list stride of the last cell seen (list sizing)
     // porosity: per sub-batch of PORO_FRAMES frames the spheres, grid headers, bit grids (zero between sub-batches) and occupied-voxel counters
     DevBuf<float4> d_poro_xyzr; DevBuf<PorosityHdr> d_poro_hdr; DevBuf<unsigned long long> d_poro_grid, d_poro_count;
+    // secondary structure: per frame of a batch the segments' atoms and CA cells, the two recorded bonds of every donor, turn / bend bits and flags
+    DevBuf<float> d_ss_res; DevBuf<float4> d_ss_hb; DevBuf<uint32_t> d_ss_bits;
 };
 
 struct Slot {
@@ -626,7 +629,7 @@ mdgpu_plan* mdgpu_plan_create_ex(const mdgpu_system_desc_t* sys, const mdgpu_pro
         for (int k = 0; k < 4; ++k) {
             if (d.idx[k] && d.idx_count[k]) {
                 pr.h_idx[k].assign(d.idx[k], d.idx[k] + d.idx_count[k]);
-                for (int32_t a : pr.h_idx[k]) if ((a < 0 && !(pr.op == MDGPU_OP_BACKBONE_ANGLES && a == -1)) || (a >= 0 && (size_t)a >= sys->num_atoms)) return bail(MDGPU_ERR_INVALID_ARG, "property '" + pr.name + "': atom index out of range");
+                for (int32_t a : pr.h_idx[k]) if ((a < 0 && !((pr.op == MDGPU_OP_BACKBONE_ANGLES || pr.op == MDGPU_OP_SECONDARY_STRUCTURE) && a == -1)) || (a >= 0 && (size_t)a >= sys->num_atoms)) return bail(MDGPU_ERR_INVALID_ARG, "property '" + pr.name + "': atom index out of range");
                 if (pr.d_idx[SPACE_FULL][k].upload(pr.h_idx[k].data(), pr.h_idx[k].size()) != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (indices)");
             }
         }
@@ -817,6 +820,22 @@ mdgpu_plan* mdgpu_plan_create_ex(const mdgpu_system_desc_t* sys, const mdgpu_pro
             }
             pr.op = MDGPU_OP_DIHEDRAL; pr.n_struct = 2 * ns; pr.backbone_segments = ns;
             e = set_temporal(pr, num_frames, 2 * ns);
+            break; }
+        case MDGPU_OP_SECONDARY_STRUCTURE: {   // (N, CA, C, O, HN) per segment, the backbone ranges in structure_offsets_b: [F, S] codes
+            const size_t ns = pr.n_struct, nr = d.num_structures_b; const uint32_t* ro = d.structure_offsets_b;
+            if (!ns) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': no backbone segments (num_structures = 0)");
+            if (pr.h_idx[0].size() != 5 * ns) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': idx[0] must hold (N, CA, C, O, HN) for each of the num_structures backbone segments");
+            for (size_t i = 0; i < 5 * ns; ++i) if (pr.h_idx[0][i] < 0 && i % 5 != 4) return bail(MDGPU_ERR_INVALID_ARG, "property '" + pr.name + "': atom index out of range");
+            if (!ro || !nr) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': no backbone range offsets (structure_offsets_b / num_structures_b)");
+            if (ro[0] != 0 || ro[nr] != ns) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': backbone range offsets must start at 0 and end at the segment count");
+            for (size_t r = 0; r < nr; ++r) if (ro[r] > ro[r + 1]) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': backbone range offsets are not ascending");
+            std::vector<uint32_t> seg(3 * ns);
+            for (size_t r = 0; r < nr; ++r) for (uint32_t i = ro[r]; i < ro[r + 1]; ++i) { seg[3 * i] = (uint32_t)r; seg[3 * i + 1] = ro[r]; seg[3 * i + 2] = ro[r + 1]; }
+            pr.h_idx[1].resize(ns); for (size_t i = 0; i < ns; ++i) pr.h_idx[1][i] = pr.h_idx[0][5 * i + 1];   // the CA atoms: the walk's AABB on open axes
+            e = pr.d_idx[SPACE_FULL][1].upload(pr.h_idx[1].data(), ns);
+            if (e == cudaSuccess) e = pr.d_ss_seg.upload(seg.data(), seg.size());
+            pr.ss_segments = ns;
+            if (e == cudaSuccess) e = set_temporal(pr, num_frames, ns);
             break; }
         case MDGPU_OP_POROSITY:   // porosity(selection): [F, 1]; an empty selection is valid and evaluates to 0 (:5896-5899)
             e = set_temporal(pr, num_frames, 1);
@@ -1052,6 +1071,10 @@ static int build_slot(mdgpu_plan* p, Slot& s, const mdgpu_unitcell_t* first_cell
             CUDA_TRY(ps.d_poro_grid.alloc((size_t)PORO_FRAMES * PORO_GRID_WORDS)); CUDA_TRY(ps.d_poro_count.alloc(PORO_FRAMES));
             CUDA_TRY(cudaMemset(ps.d_poro_grid.get(), 0, ps.d_poro_grid.bytes()));
             CUDA_TRY(cudaMemset(ps.d_poro_count.get(), 0, ps.d_poro_count.bytes()));
+        } else if (pr.op == MDGPU_OP_SECONDARY_STRUCTURE) {
+            CUDA_TRY(ps.d_geom.alloc(p->B)); CUDA_TRY(ps.d_aabb.alloc((size_t)6 * p->B));
+            CUDA_TRY(ps.d_ss_res.alloc((size_t)p->B * pr.ss_segments * SS_RES_FLOATS));
+            CUDA_TRY(ps.d_ss_hb.alloc((size_t)p->B * pr.ss_segments)); CUDA_TRY(ps.d_ss_bits.alloc((size_t)p->B * 2 * pr.ss_segments));
         } else if (pr.op == MDGPU_OP_RMSD) {
             CUDA_TRY(ps.d_sdf_xyzw.alloc((size_t)p->B * 2 * pr.h_idx[0].size()));   // [B][initial, current][atoms]
         } else if (pr.op == MDGPU_OP_PLANE || pr.op == MDGPU_OP_SHAPE_WEIGHTS) {
@@ -1152,6 +1175,21 @@ template <typename F> static void timed_launch(mdgpu_plan* p, cudaStream_t st, i
     if (p->timing) { cudaEventCreate(&tl.a); cudaEventCreate(&tl.b); cudaEventRecord(tl.a, st); }
     launch();
     if (p->timing) { cudaEventRecord(tl.b, st); p->timed.push_back(tl); }
+}
+
+// md_spatial_acc_init(&acc, CA, 9.0, cell) and its pair walk at cutoff 9.0 (md_util.c:2122, 2150)
+constexpr double SS_CUTOFF = 9.0;
+// why the candidate walk of a frame with this cell cannot be restated (nullptr: it can). A triclinic cell must be periodic on all axes
+// (md_spatial_acc.c:201-202) and not degenerate; a periodic axis needs at least 2n + 1 cells for the neighbour reach n, so that no pair of cells
+// is joined by two offsets (a narrower cell could report a pair twice).
+static const char* ss_cell_unsupported(const mdgpu_unitcell_t& c) {
+    if ((c.flags & MDGPU_CELL_TRICLINIC) && (c.flags & MDGPU_CELL_PBC_ALL) != MDGPU_CELL_PBC_ALL) return "a triclinic cell must be periodic on all axes";
+    FrameGeom g; host_frame_geom(&g, &c, SS_CUTOFF, SS_CUTOFF, nullptr, 0xffffffffu);
+    if ((c.flags & MDGPU_CELL_TRICLINIC) && g.valid <= 0) return "degenerate triclinic cell";
+    for (int k = 0; k < 3; ++k)
+        if ((c.flags & (MDGPU_CELL_PBC_X << k)) && (g.ncell[k] > 2 || g.cdim[k] < 2 * g.ncell[k] + 1))
+            return "a periodic axis of the cell is too narrow for the 9 A candidate search to visit each residue pair once (at least 27 A, or wider when skewed)";
+    return nullptr;
 }
 
 // enqueue the property kernels of one batch whose frames are already in device memory, in atom space `sp`: SPACE_COMPACT when host ingest
@@ -1307,6 +1345,20 @@ static int enqueue_batch(mdgpu_plan* p, Slot& s, const BatchFrames& fr, uint32_t
                 launch_porosity(a, (int)nf, s.stream);
             }
             break;
+        case MDGPU_OP_SECONDARY_STRUCTURE: {
+            for (int i = 0; i < B; ++i) {   // the walk must reach each pair of cells by one offset (see dssp.cu); periodic axes decide it without the data
+                const mdgpu_unitcell_t& c = s.h_cells[i];
+                const char* why = ss_cell_unsupported(c);
+                if (why) return fail(MDGPU_ERR_UNSUPPORTED, "secondary structure '%s': frame %u: %s", pr.name.c_str(), frame0 + i, why);
+            }
+            const float* aabb = nullptr;
+            if (!all_pbc) { launch_aabb(fr, didx[1], (uint32_t)pr.ss_segments, ps.d_aabb.get(), s.stream); aabb = ps.d_aabb.get(); }
+            launch_geom(s.d_cells.get(), aabb, ps.d_geom.get(), SS_CUTOFF, SS_CUTOFF, 0xffffffffu, B, s.d_err.get(), s.stream);
+            SsArgs a{};
+            a.frames = fr; a.atoms = didx[0]; a.seg = pr.d_ss_seg.get(); a.S = (uint32_t)pr.ss_segments; a.geom = ps.d_geom.get();
+            a.res = ps.d_ss_res.get(); a.hb = ps.d_ss_hb.get(); a.bits = ps.d_ss_bits.get(); a.out = pr.d_temporal.get(); a.frame0 = frame0; a.err = s.d_err.get();
+            launch_secondary_structure(a, B, tri, s.stream);
+            break; }
         case MDGPU_OP_RMSD: {
             if (!p->have_init) return fail(MDGPU_ERR_INVALID_ARG, "rmsd '%s' needs the initial frame (mdgpu_plan_set_initial_frame)", pr.name.c_str());
             RmsdArgs a{};
@@ -1367,6 +1419,7 @@ static int publish_batch(mdgpu_plan* p, uint32_t beg, uint32_t cnt);
 static int device_error(mdgpu_plan* p, int err) {
     if (err == MDGPU_ERR_CAPACITY) return fail(err, "a frame needs more cells than the plan reserved from its first frame (cell capacity %u); raise mdgpu_plan_options_t.cell_capacity", p->cell_cap);
     if (err == MDGPU_ERR_FRAME_SOURCE) return fail(err, "XTC: Failed to decode frame data (%d)", err);
+    if (err == MDGPU_ERR_UNSUPPORTED) return fail(err, "a property kernel found a frame outside what it supports (device-side check; the unit cells of the batch are the usual cause)");
     return fail(err, "device-side error %d", err);
 }
 
@@ -2095,6 +2148,22 @@ int mdgpu_plan_rama_density(mdgpu_plan* p, size_t prop, const uint32_t* segments
     if (cudaMemcpy(out_tex, a.buf[1], sizeof(float) * texels, cudaMemcpyDeviceToHost) != cudaSuccess || cudaMemcpy(samples, d_samples.get(), sizeof(samples), cudaMemcpyDeviceToHost) != cudaSuccess)
         return fail(MDGPU_ERR_CUDA, "rama density failed: %s", cudaGetErrorString(cudaGetLastError()));
     for (int c = 0; c < 4; ++c) out_sum[c] = (float)(double)samples[c];   // den_sum: (float) of the task's double sum
+    return 0;
+}
+
+int mdgpu_plan_secondary_structure(mdgpu_plan* p, size_t prop, uint32_t frame_beg, uint32_t frame_end, int32_t* out) {
+    if (!p || prop >= p->props.size()) return fail(MDGPU_ERR_INVALID_ARG, "mdgpu_plan_secondary_structure: invalid argument");
+    Prop& pr = p->props[prop];
+    if (!pr.ss_segments) return fail(MDGPU_ERR_INVALID_ARG, "property '%s' is not a secondary-structure property", pr.name.c_str());
+    if (!out && frame_end > frame_beg) return fail(MDGPU_ERR_INVALID_ARG, "mdgpu_plan_secondary_structure: no output array");
+    if (frame_beg > frame_end || frame_end > p->num_frames) return fail(MDGPU_ERR_INVALID_ARG, "mdgpu_plan_secondary_structure: frame range [%u, %u) outside [0, %zu)", frame_beg, frame_end, p->num_frames);
+    int rc = mdgpu_plan_sync(p); if (rc) return rc;   // multi-device plans hold every frame's rows on devices[0] = p->device from here on
+    if (frame_end == frame_beg) return 0;
+    CUDA_TRY(cudaSetDevice(p->device));
+    const size_t n = (size_t)(frame_end - frame_beg) * pr.ss_segments;
+    std::vector<float> rows(n);
+    CUDA_TRY(cudaMemcpy(rows.data(), pr.d_temporal.get() + (size_t)frame_beg * pr.ss_segments, sizeof(float) * n, cudaMemcpyDeviceToHost));
+    for (size_t k = 0; k < n; ++k) out[k] = (int32_t)rows[k];   // rows of frames not evaluated are 0 (MD_SECONDARY_STRUCTURE_UNKNOWN)
     return 0;
 }
 
