@@ -145,6 +145,15 @@ typedef enum mdgpu_op {
  *              system-wide cell list (get_spatial_acc :734); so far its only consumer on the device is count().
  *              count(<coordinate range> [and static]): a mdgpu_range_arg_t for argument 0, its static side in dyn[0], idx[0] empty and
  *              cutoff_min = cutoff_max = 0; the count of the frame's selected atoms (_count :2868).
+ *              count(x, 'residue' | 'chain' | 'structure') (_count_with_arg -> internal_count :5465-5531): bit 1 of com_args set = the value of a
+ *              frame is the number of groups that hold at least one atom of the frame's selection (the selection count(x) counts: within() minus
+ *              its own selection, or the range, `and` its static side). The groups are num_structures lists of atoms in idx[1], delimited by
+ *              structure_offsets[num_structures + 1], or structure_size atoms each when that pointer is NULL; num_structures = 0 is valid and
+ *              gives 0 in every frame. The reference's groups are the components (md_system_component_atom_range) for 'residue', the instances
+ *              (md_system_instance_atom_range) for 'chain', and the bond-connected structures (md_util_system_infer_structures) for 'structure'.
+ *              idx[0], idx[2], cutoff_*, dyn[0] and the range argument keep their meaning; 'atom' is count(x) itself, bit 1 clear. mdgpu_plan_create
+ *              fails with MDGPU_ERR_INVALID_ARG for an atom out of range, an atom in two groups, and offsets that do not rise from 0 to idx_count[1].
+ *              The value is a float holding the exact integer count.
  *   SHAPE_WEIGHTS: idx[0] = the atoms of num_structures structures back to back (structure_offsets, or structure_size each), bit 0 of com_args
  *              = weights are the atom masses (shapespace's use_mass; _shape_weights always uses them), else 1.
  *   COORD_X/_Y/_Z: idx[0] = the atoms.
@@ -219,7 +228,8 @@ typedef struct mdgpu_property_desc_t {
     float cutoff_min;
     float cutoff_max;
     const uint32_t* structure_offsets;   /* optional CSR offsets into idx[0] for groups of different sizes (rdf) */
-    uint32_t com_args;                   /* distance/angle/dihedral: bit k = argument k is a selection (centre of mass even for one atom) */
+    uint32_t com_args;                   /* distance/angle/dihedral: bit k = argument k is a selection (centre of mass even for one atom); WITHIN_COUNT:
+                                          * bit 0 = idx[2] is a static `and` side, bit 1 = count over the groups of idx[1] (see above) */
     float ref_within_radius;             /* rdf: > 0 -> the reference argument was within(radius, idx[0]): the dynamic selection is evaluated per frame */
     float ref_within_min;                /* ... within(min:radius, idx[0]) (_within_expl_frng :2609); 0 for the plain form */
     const uint32_t* structure_offsets_b; /* distance_pair: CSR groups of argument 1 when it was an array of selections (argument 0 uses structure_offsets);

@@ -5,7 +5,7 @@ the thin host-side mirror of the md_script evaluation API used by the tests and 
 """
 from .api import (  # noqa: F401
     MdgpuError, UnitCell, System, Property, PropertyData, Plan, Within, Range, Trajectory, ArrayTrajectory,
-    rdf, rdf_com, rdf_within, sdf, density, distance, distance_min, distance_max, distance_pair, rmsd, porosity, com, plane, count_within, count_range, in_contexts, shape_weights, coord, angle, dihedral, expression, backbone_angles, secondary_structure, contact_count, water_system, device_count, bind_host_to_device, launch_count, lib,
+    rdf, rdf_com, rdf_within, sdf, density, distance, distance_min, distance_max, distance_pair, rmsd, porosity, com, plane, count_within, count_range, count_groups, count_groups_of, COUNT_TYPES, in_contexts, shape_weights, coord, angle, dihedral, expression, backbone_angles, secondary_structure, contact_count, water_system, device_count, bind_host_to_device, launch_count, lib,
     synth_membrane_desc, synth_membrane_base, synth_membrane_frames_host, synth_membrane_frames_device, membrane_system,
     synth_water_desc, synth_water_base, synth_water_frames_host, synth_water_frames_device,
     xtc_frame_offsets, xtc_decode_frames,

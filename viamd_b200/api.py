@@ -233,6 +233,8 @@ class System:
     resname: Optional[Sequence[str]] = None        # per residue
     res_atom_offset: Optional[np.ndarray] = None   # [num_res + 1]
     radius: Optional[np.ndarray] = None            # van der Waals radii (md_atom_extract_radii); required by porosity()
+    chain_atom_range: Optional[np.ndarray] = None  # [num_chains, 2] (first atom, one past the last) of each instance (md_system_instance_atom_range);
+                                                   # required by count(x, 'chain')
 
 
 @dataclass
@@ -448,6 +450,49 @@ def count_range(name, rng: Range):
     """count(within_x / _y / _z / _xyz(...) [and static]): per frame the number of atoms in the coordinate range (coordinate_range
     md_script_functions.inl:2394, _count :2868) — MDGPU_OP_WITHIN_COUNT with the range as dyn[0]"""
     return Property(name, OP_WITHIN_COUNT, [np.zeros(0, np.int32)], ranges={0: rng})
+
+
+COUNT_TYPES = ("atom", "residue", "chain", "structure")   # count_type_str (md_script_functions.inl:5448-5452); 'chain' counts instances
+
+
+def count_groups_of(system: System, count_type: str) -> list:
+    """the groups count(x, count_type) counts over (internal_count md_script_functions.inl:5465-5531), as atom index arrays:
+    'residue' the residues of System.res_atom_offset, 'chain' the instances of System.chain_atom_range, 'structure' the connected components of
+    the bond graph in the order md_util_system_infer_structures finds them (a breadth-first walk from every atom not yet visited; an atom without
+    bonds is a structure of its own, and a system without bonds has no structures)."""
+    if count_type == "residue":
+        off = np.asarray(system.res_atom_offset, np.int64)
+        return [np.arange(off[i], off[i + 1], dtype=np.int32) for i in range(len(off) - 1)]
+    if count_type == "chain":
+        if system.chain_atom_range is None: raise ValueError("count(x, 'chain'): the system has no chain atom ranges (System.chain_atom_range)")
+        return [np.arange(int(b), int(e), dtype=np.int32) for b, e in np.asarray(system.chain_atom_range, np.int64).reshape(-1, 2)]
+    if count_type == "structure":
+        if system.conn_offset is None or len(system.conn_idx) == 0: return []
+        co = np.asarray(system.conn_offset, np.int64); ci = np.asarray(system.conn_idx, np.int64)
+        seen = np.zeros(system.num_atoms, bool); out = []
+        for i in range(system.num_atoms):
+            if seen[i]: continue
+            seen[i] = True; order = [i]; head = 0
+            while head < len(order):
+                a = order[head]; head += 1
+                for b in ci[co[a]:co[a + 1]] if a + 1 < len(co) else ():
+                    if not seen[b]: seen[b] = True; order.append(int(b))
+            out.append(np.asarray(order, np.int32))
+        return out
+    raise ValueError(f"unknown count type {count_type!r}; valid types are {', '.join(COUNT_TYPES)}")
+
+
+def count_groups(name, sel, groups):
+    """count(x, 'residue' | 'chain' | 'structure'): per frame the number of groups (atom index arrays, each atom in at most one) that hold an
+    atom of the dynamic selection x — Within(...) or Range(...), optionally with its static `and` side (internal_count md_script_functions.inl:5465).
+    MDGPU_OP_WITHIN_COUNT with bit 1 of com_args: the groups back to back in idx[1], their CSR offsets in structure_offsets."""
+    base = count_range(name, sel) if isinstance(sel, Range) else count_within(name, sel.radius, sel.sel, sel.radius_min, sel.and_idx)
+    groups = [np.asarray(g, np.int32) for g in groups]
+    off = np.zeros(len(groups) + 1, np.uint32); off[1:] = np.cumsum([len(g) for g in groups])
+    idx = list(base.idx) + [np.zeros(0, np.int32)] * (2 - len(base.idx))
+    idx[1] = np.concatenate(groups).astype(np.int32) if off[-1] else np.zeros(0, np.int32)
+    base.idx = idx; base.com_args |= 2; base.num_structures = len(groups); base.structure_offsets = off
+    return base
 
 
 def shape_weights(name, groups, use_mass=True):

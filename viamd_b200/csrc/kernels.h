@@ -105,6 +105,13 @@ void launch_rmsd_groups(const RmsdArgs& a, int B, cudaStream_t s);   // one valu
 void launch_plane(const RmsdArgs& a, int B, cudaStream_t s);   // plane(selection): out is [num_frames][4], scratch [B][n], init_xyz unused
 
 // within.cu — count(within(radius, selection))
+// count(x, 'residue' | 'chain' | 'structure'): the groups the count is over, as a map atom -> group (-1: in no group) and per frame of the
+// batch one hit byte per group. group_of == null: count the atoms (count(x), count(x, 'atom')).
+struct GroupArgs {
+    const int32_t* group_of;         // [num_atoms]
+    uint8_t* hits;                   // [B][n_groups]
+    uint32_t n_groups;
+};
 struct WithinArgs {
     const FrameGeom* geom;           // grid of ALL atoms: cell extent ceil(radius/6)*6, cutoff = radius (get_spatial_acc)
     CellList trg, ref;               // all atoms (clamped cells) / the selection's atoms (home grid)
@@ -115,6 +122,7 @@ struct WithinArgs {
     uint8_t* flags;                  // [B][num_atoms], zeroed by the launcher
     float* out;                      // [num_frames]
     uint32_t frame0;
+    GroupArgs grp;                   // count over groups of atoms (k_group_count), or group_of == null
 };
 void launch_within_count(const WithinArgs& a, int B, bool tri, int sm_count, cudaStream_t s);
 // the same marks as a per-frame ascending index list (dyn_idx [B][num_atoms], dyn_n [B]); consumers take it as a DynSel
@@ -129,7 +137,7 @@ struct RangeArgs {
     uint8_t* flags;                  // [B][num_atoms]
 };
 void launch_range_list(const RangeArgs& a, int B, int sm_count, int32_t* d_dyn_idx, uint32_t* d_dyn_n, cudaStream_t s);
-void launch_range_count(const RangeArgs& a, int B, int sm_count, float* d_out, uint32_t frame0, cudaStream_t s);
+void launch_range_count(const RangeArgs& a, const GroupArgs& g, int B, int sm_count, float* d_out, uint32_t frame0, cudaStream_t s);
 void launch_scan_home_cells(const FrameGeom* d_geom, const CellList& cl, int B, cudaStream_t s);   // cells.cu: k_scan_cells<1> alone
 
 // props.cu

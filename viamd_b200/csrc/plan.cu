@@ -116,6 +116,8 @@ struct Prop {
     std::vector<uint32_t> h_goff[2]; DevBuf<uint32_t> d_goff[2];   // argument 0 / 1 is an ARRAY of selections, one position per selection: their CSR offsets in idx[k]
     std::vector<uint32_t> h_aoff[4]; DevBuf<uint32_t> d_aoff[4];   // distance / angle / dihedral / com: argument k is an ARRAY of selections (centre of their centres)
     DevBuf<uint8_t> d_and_mask;   // `selection and within(...)`: one byte per atom of the static side (count(within()) / rdf(within()))
+    // count(x, 'residue' | 'chain' | 'structure') (com_args bit 1): the group of every atom (-1: none) and the number of groups
+    DevBuf<int32_t> d_group_of; uint32_t n_groups = 0; bool count_groups = false;
     // Dynamic arguments: argument k is within([rmin:]rmax, h_idx[k]) [and a static selection], evaluated per frame on the device into an ascending
     // index list (md_script_functions.inl:2485-2720); the consumers read that list instead of the static one. A coordinate range (`range`:
     // within_x / _y / _z / _xyz, coordinate_range :2394) marks the atoms inside [lo, hi] instead, testing only the static side's atoms (d_and_idx)
@@ -171,7 +173,8 @@ struct Prop {
 
 // One within([rmin:]rmax, selection) query per frame of a batch: the system-wide grid and the cell lists of all atoms and of the selection
 // (get_spatial_acc :734), the marks [B][num_atoms] and, for a dynamic argument, the per-frame index list (empty for count(within())).
-struct WithinScratch { DevBuf<FrameGeom> d_geom; DevBuf<float> d_aabb; CellListBuf trg, ref; DevBuf<uint8_t> d_flags; DevBuf<int32_t> d_idx; DevBuf<uint32_t> d_n; };
+// count over groups of atoms also takes one hit byte per group and frame (d_hits [B][n_groups]).
+struct WithinScratch { DevBuf<FrameGeom> d_geom; DevBuf<float> d_aabb; CellListBuf trg, ref; DevBuf<uint8_t> d_flags; DevBuf<int32_t> d_idx; DevBuf<uint32_t> d_n; DevBuf<uint8_t> d_hits; };
 
 struct PropScratch {   // per (stream slot, property)
     DevBuf<FrameGeom> d_geom; DevBuf<float> d_aabb;
@@ -405,6 +408,28 @@ static std::string take_structures(Prop& pr, const mdgpu_property_desc_t& d, con
     else if (!pr.struct_size) return who + ": structure_size or structure_offsets required";
     else { pr.h_soff.resize(pr.n_struct + 1); for (size_t k = 0; k <= pr.n_struct; ++k) pr.h_soff[k] = (uint32_t)(k * pr.struct_size); }
     return check_offsets(pr.h_soff.data(), pr.n_struct, pr.h_idx[0].size(), who, "structure offsets", "idx[0]");
+}
+
+// count(x, 'residue' | 'chain' | 'structure'): the num_structures groups of idx[1] (structure_offsets, or runs of structure_size atoms) as the
+// map atom -> group in pr.d_group_of; every atom in at most one group. "" or the error message (*e: a failed upload)
+static std::string take_count_groups(Prop& pr, const mdgpu_property_desc_t& d, size_t num_atoms, cudaError_t* e) {
+    const std::string who = "'" + pr.name + "'";
+    const size_t n = d.num_structures;
+    if (n >= (size_t)INT32_MAX) return who + ": too many groups";
+    std::vector<uint32_t> off(n + 1);
+    if (d.structure_offsets) off.assign(d.structure_offsets, d.structure_offsets + n + 1);
+    else for (size_t k = 0; k <= n; ++k) off[k] = (uint32_t)(k * d.structure_size);
+    const std::string er = check_offsets(off.data(), n, pr.h_idx[1].size(), who, "group offsets", "idx[1]"); if (!er.empty()) return er;
+    std::vector<int32_t> group_of(num_atoms, -1);
+    for (size_t g = 0; g < n; ++g)
+        for (uint32_t j = off[g]; j < off[g + 1]; ++j) {
+            int32_t& slot = group_of[(size_t)pr.h_idx[1][j]];   // in range: idx lists are checked when they are taken
+            if (slot >= 0) return who + ": atom " + std::to_string(pr.h_idx[1][j]) + " is in two groups";
+            slot = (int32_t)g;
+        }
+    pr.n_groups = (uint32_t)n; pr.count_groups = true;
+    *e = pr.d_group_of.upload(group_of.data(), group_of.size());
+    return std::string();
 }
 
 // a temporal of `len` values per frame: device rows, host values and, for len > 1, the per-frame aggregates (allocate_property_data :5618-5640)
@@ -753,6 +778,10 @@ mdgpu_plan* mdgpu_plan_create_ex(const mdgpu_system_desc_t* sys, const mdgpu_pro
             e = set_temporal(pr, num_frames, len);
             break; }
         case MDGPU_OP_WITHIN_COUNT:   // count(within(radius, selection)); an empty selection is valid (nothing is within reach of nothing). count(<range>): dyn[0]
+            if (d.com_args & 2u) {   // count(x, 'residue' | 'chain' | 'structure'): the groups in idx[1]
+                const std::string er = take_count_groups(pr, d, sys->num_atoms, &e); if (!er.empty()) return bail(MDGPU_ERR_INVALID_ARG, er);
+                if (e != cudaSuccess) return bail(MDGPU_ERR_CUDA, "device allocation failed (atom groups)");
+            }
             if (pr.dyn[0].range) { e = set_temporal(pr, num_frames, 1); break; }
             if (!(pr.cutoff_max > 0.0f)) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': The supplied radius is negative or zero, please supply a positive value");   // :2528
             if (pr.cutoff_min < 0.0f || pr.cutoff_max < pr.cutoff_min) return bail(MDGPU_ERR_INVALID_ARG, "'" + pr.name + "': The supplied radius range is invalid");          // :2654
@@ -1064,8 +1093,9 @@ static int build_slot(mdgpu_plan* p, Slot& s, const mdgpu_unitcell_t* first_cell
             CUDA_TRY(ps.d_sdf_xyzw.alloc((size_t)p->B * (pr.n_struct + 1) * pr.struct_size));
             CUDA_TRY(ps.d_sdf_ref0.alloc((size_t)p->B * 20));
             CUDA_TRY(ps.d_sdf_mats.alloc((size_t)p->B * pr.n_struct * 32));
-        } else if (pr.op == MDGPU_OP_WITHIN_COUNT && !pr.dyn[0].on) {
-            const int rc = alloc_within(p, ps.within[0], pr.h_idx[0].size(), cap, false); if (rc) return rc;
+        } else if (pr.op == MDGPU_OP_WITHIN_COUNT) {   // a range's scratch was allocated with the dynamic arguments above
+            if (!pr.dyn[0].on) { const int rc = alloc_within(p, ps.within[0], pr.h_idx[0].size(), cap, false); if (rc) return rc; }
+            if (pr.count_groups) CUDA_TRY(ps.within[0].d_hits.alloc((size_t)p->B * pr.n_groups));   // count over groups: one hit byte per group and frame
         } else if (pr.op == MDGPU_OP_POROSITY) {
             CUDA_TRY(ps.d_poro_xyzr.alloc((size_t)PORO_FRAMES * pr.h_idx[0].size())); CUDA_TRY(ps.d_poro_hdr.alloc(PORO_FRAMES));
             CUDA_TRY(ps.d_poro_grid.alloc((size_t)PORO_FRAMES * PORO_GRID_WORDS)); CUDA_TRY(ps.d_poro_count.alloc(PORO_FRAMES));
@@ -1299,9 +1329,10 @@ static int enqueue_batch(mdgpu_plan* p, Slot& s, const BatchFrames& fr, uint32_t
             timed_launch(p, s.stream, 2, [&] { launch_density(a, B, s.stream); });
             break; }
         case MDGPU_OP_WITHIN_COUNT: {
-            if (pr.dyn[0].on) { launch_range_count(range_args(p, pr.dyn[0], ps.within[0], fr), B, p->sm_count, pr.d_temporal.get(), frame0, s.stream); break; }
+            const GroupArgs grp{ pr.count_groups ? pr.d_group_of.get() : nullptr, ps.within[0].d_hits.get(), pr.n_groups };
+            if (pr.dyn[0].on) { launch_range_count(range_args(p, pr.dyn[0], ps.within[0], fr), grp, B, p->sm_count, pr.d_temporal.get(), frame0, s.stream); break; }
             WithinArgs a = enqueue_within(p, s, ps.within[0], fr, all_pbc, didx[0], pr.h_idx[0].size(), pr.cutoff_min, pr.cutoff_max, pr.d_and_mask.get(), frame0);
-            a.out = pr.d_temporal.get();
+            a.out = pr.d_temporal.get(); a.grp = grp;
             launch_within_count(a, B, tri, p->sm_count, s.stream);
             break; }
         case MDGPU_OP_COM: {

@@ -76,6 +76,47 @@ __global__ void __launch_bounds__(256) k_within_count(WithinArgs a) {
     if (threadIdx.x == 0) a.out[a.frame0 + f] = (float)total;
 }
 
+// count(x, 'residue' | 'chain' | 'structure') (_count_with_arg -> internal_count md_script_functions.inl:5465-5531): per frame the number of
+// groups that hold at least one atom of the selection k_within_count counts. One CTA per frame in three phases, separated by barriers:
+//   1. the frame's hit bytes are zeroed and the within() selection's own atoms leave the marks (:2524);
+//   2. every marked atom that passes the static `and` side sets the hit byte of its group (idempotent: the stores' order does not matter);
+//   3. the set hit bytes are counted.
+// O(atoms + groups) per frame whatever the groups' layout; the count is an exact integer.
+constexpr int GROUP_THREADS = 1024;
+__global__ void __launch_bounds__(GROUP_THREADS) k_group_count(WithinArgs a) {
+    const int f = blockIdx.x;
+    uint8_t* __restrict__ flags = a.flags + (size_t)f * a.num_atoms;
+    uint8_t* __restrict__ hits = a.grp.hits + (size_t)f * a.grp.n_groups;
+    const int32_t* __restrict__ group_of = a.grp.group_of;
+    __shared__ uint32_t total;
+    if (threadIdx.x == 0) total = 0;
+    for (uint32_t g = threadIdx.x; g < a.grp.n_groups; g += blockDim.x) hits[g] = 0;
+    for (uint32_t k = threadIdx.x; k < a.n_sel; k += blockDim.x) flags[a.sel[k]] = 0;
+    __syncthreads();
+    for (uint32_t i = threadIdx.x; i < a.num_atoms; i += blockDim.x) {
+        if (!flags[i] || (a.and_mask && !a.and_mask[i])) continue;
+        const int32_t g = group_of[i];
+        if (g >= 0) hits[g] = 1;
+    }
+    __syncthreads();
+    uint32_t c = 0;
+    for (uint32_t g = threadIdx.x; g < a.grp.n_groups; g += blockDim.x) c += hits[g];
+    if (c) atomicAdd(&total, c);
+    __syncthreads();
+    if (threadIdx.x == 0) a.out[a.frame0 + f] = (float)total;
+}
+
+// the per-frame count of the marks: of the atoms, or of the groups they fall in
+static void launch_count(const WithinArgs& a, int B, cudaStream_t s) {
+    if (a.grp.group_of) {
+        k_group_count<<<B, GROUP_THREADS, 0, s>>>(a);
+        note_launch("k_group_count", s);
+    } else {
+        k_within_count<<<B, 256, 0, s>>>(a);
+        note_launch("k_within_count", s);
+    }
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 // The dynamic selection as the REFERENCE set of an rdf(): rdf(within(radius, selection), targets, cutoff). The marked atoms (selection
 // removed) become a per-frame index list; its reference cell list is built like cells.cu builds a static one, but with the frame's own
@@ -127,8 +168,7 @@ void launch_within_list(const WithinArgs& a, int B, bool tri, int sm_count, int3
 void launch_within_count(const WithinArgs& a, int B, bool tri, int sm_count, cudaStream_t s) {
     if (B <= 0) return;
     launch_mark(a, B, tri, sm_count, s);
-    k_within_count<<<B, 256, 0, s>>>(a);
-    note_launch("k_within_count", s);
+    launch_count(a, B, s);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -175,12 +215,11 @@ void launch_range_list(const RangeArgs& a, int B, int sm_count, int32_t* d_dyn_i
     note_launch("k_within_compact", s);
 }
 
-void launch_range_count(const RangeArgs& a, int B, int sm_count, float* d_out, uint32_t frame0, cudaStream_t s) {
+void launch_range_count(const RangeArgs& a, const GroupArgs& g, int B, int sm_count, float* d_out, uint32_t frame0, cudaStream_t s) {
     if (B <= 0) return;
     WithinArgs w = range_mark(a, B, sm_count, s);
-    w.out = d_out; w.frame0 = frame0;
-    k_within_count<<<B, 256, 0, s>>>(w);
-    note_launch("k_within_count", s);
+    w.out = d_out; w.frame0 = frame0; w.grp = g;
+    launch_count(w, B, s);
 }
 
 }  // namespace mdg

@@ -9,6 +9,7 @@ Supported statements:  ident = proc(args);   with proc in
     rdf(sel, sel, cutoff | min:max)   sdf(residue(a:b) | sel-array, sel, cutoff)   density_x|_y|_z(sel)
     distance(i, j)   angle(i, j, k)   dihedral(i, j, k, l)            (1-based atom indices as in md_script)
     porosity(sel)                                                        (needs System.radius)
+    count(dyn [, 'atom' | 'residue' | 'chain' | 'structure'])           (dyn: a dynamic selection below; 'chain' needs System.chain_atom_range)
 and temporal expressions: + - * / and unary -, the functions sqrt cbrt abs floor ceil cos sin asin acos atan log exp log2 exp2 log10
 atan(y, x) atan2 pow min max, over numbers, PI / TAU / E, earlier temporal properties and inline calls of the procedures above.
 Selections (evaluated once, statically, to ascending atom index lists — md_script.c:5492-5524):
@@ -406,10 +407,17 @@ class _Parser:
             a = self.groups_or_selection(); self.expect("ch", ","); b = self.selection(); self.expect("ch", ","); c = self.number()
             if self.peek() == ("ch", ","): raise ScriptError("Could not find matching procedure 'contact_count' which takes four arguments")
             p = api.contact_count(ident, a if isinstance(a, list) else [a], b, c, self.sys, 4)
-        elif proc == "count":   # count(<dynamic selection>): the selection is evaluated per frame on the device
+        elif proc == "count":   # count(<dynamic selection> [, 'atom' | 'residue' | 'chain' | 'structure']): the selection is evaluated per frame on the device
             if not self._has_within_before_comma(): raise ScriptError("count() is lowered for within(...) and within_x / _y / _z / _xyz(...) expressions only")
-            d = self.dyn_arg()
-            p = api.count_range(ident, d) if isinstance(d, api.Range) else api.count_within(ident, d.radius, d.sel, d.radius_min, d.and_idx)
+            d = self.dyn_arg(); kind = "atom"
+            if self.peek() == ("ch", ","):   # _count_with_arg (md_script_functions.inl:5536): an unknown type fails at compile time
+                self.next(); kind = self.expect("str")[1]
+                if kind not in api.COUNT_TYPES: raise ScriptError(f"Unknown argument: '{kind}', valid arguments are: {', '.join(api.COUNT_TYPES)}")
+            if kind == "atom": p = api.count_range(ident, d) if isinstance(d, api.Range) else api.count_within(ident, d.radius, d.sel, d.radius_min, d.and_idx)
+            else:
+                try: groups = api.count_groups_of(self.sys, kind)
+                except ValueError as e: raise ScriptError(str(e)) from None
+                p = api.count_groups(ident, d, groups)
         elif proc in ("coord_x", "coord_y", "coord_z"):
             a = self.index()   # an array of selections: one value per selection (its centre of mass, coordinate_extract :1503)
             p = api.coord(ident, "xyz".index(proc[-1]), a if isinstance(a, list) else ([a] if np.ndim(a) == 0 else a))
