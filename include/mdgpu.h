@@ -263,7 +263,10 @@ typedef struct mdgpu_plan_options_t {
     uint32_t batch_frames;        /* frames per launch batch; 0 = default (one per SM) */
     uint32_t num_streams;         /* CUDA streams (slots) the frame loop is dispatched onto; 0 = default (6), at most 8 */
     uint32_t keep_frame_results;  /* 1: retain raw per-frame integer bins of distributions (parity tests) */
-    uint32_t cell_capacity;       /* cells per frame the cell lists are sized for; 0 = 2x the initial frame's grid */
+    uint32_t cell_capacity;       /* cells per frame the cell lists are sized for; 0 = 2x the grid of the first evaluation's first frame, at least
+                                   * 2^16. A non-periodic axis (no cell, or a cell without PBC on it) gets its grid from the atoms' bounding box:
+                                   * mdgpu_eval_host_frames fits it to all frames of that call; device-resident, XTC and trajectory frames are not
+                                   * seen then and get 2^16. A frame that needs more cells fails its batch with MDGPU_ERR_CAPACITY; raise this */
     uint32_t rdf_variant;         /* rdf pair-kernel variant, all bit-identical in their results: 0 = default (register-pair targets, 4 CTAs/SM), 1 = scalar kernel
                                    * without candidate lists, 2 = 3 CTAs/SM with a longer hit queue, 4 = reference chunks staged by the TMA unit
                                    * (cp.async.bulk + mbarrier; kept as an alternative) */

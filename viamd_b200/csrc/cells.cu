@@ -199,11 +199,13 @@ __global__ void k_bin_points(BatchFrames fr, const int32_t* __restrict__ idx_, c
     cl.rank[o] = atomicAdd(&cl.cell_cnt[(size_t)f * (cl.cap + 1) + cell], 1u);
 }
 
-// exclusive scan of the per-cell counts, one CTA per frame; writes offsets in place, total at [num]
+// exclusive scan of the per-cell counts, one CTA per frame; writes offsets in place, total at [num]. A frame over the cell capacity
+// (valid < 0) has more cells than its cap + 1 entries: it scans no cell, so only its entry 0 is written (0, where k_bin_points parked its
+// points) and k_scatter_points keeps them inside the frame; no consumer reads such a frame's list.
 template <int MODE>
 __global__ void k_scan_cells(const FrameGeom* __restrict__ geom, CellList cl) {
     const int f = blockIdx.x;
-    const uint32_t num = (MODE == 0) ? geom[f].num_cells : geom[f].num_home;
+    const uint32_t num = geom[f].valid < 0 ? 0u : (MODE == 0) ? geom[f].num_cells : geom[f].num_home;
     uint32_t* cnt = cl.cell_cnt + (size_t)f * (cl.cap + 1);
     __shared__ uint32_t warp_sums[32];
     __shared__ uint32_t carry;

@@ -1119,18 +1119,34 @@ static int build_slot(mdgpu_plan* p, Slot& s, const mdgpu_unitcell_t* first_cell
     return 0;
 }
 
+// The frames of the evaluation that builds the slots, when they are in host memory: a grid fitted to them sizes the default cell capacity.
+struct FitFrames { const float* xyz; size_t frame_stride, axis_stride; uint32_t count; };
+
+// min[3], max[3] over every atom of every frame, starting from the origin as k_aabb does: it holds the box each frame's grid is fitted to
+static void fit_frames_aabb(const FitFrames& fr, size_t num_atoms, float box[6]) {
+    for (int k = 0; k < 6; ++k) box[k] = 0.0f;
+    for (uint32_t f = 0; f < fr.count; ++f) for (int k = 0; k < 3; ++k) {
+        const float* v = fr.xyz + (size_t)f * fr.frame_stride + (size_t)k * fr.axis_stride;
+        for (size_t i = 0; i < num_atoms; ++i) { box[k] = fminf(box[k], v[i]); box[3 + k] = fmaxf(box[3 + k], v[i]); }
+    }
+}
+
 // slot set-up (lazy: needs the first frame's cell for the default cell capacity). All or nothing: the slots and each slot's host staging
 // become the plan's only once all their allocations have succeeded; after a failure the owners free what was built and the next call
 // builds again.
-static int ensure_slots(mdgpu_plan* p, const mdgpu_unitcell_t* first_cell, bool need_host_staging) {
+static int ensure_slots(mdgpu_plan* p, const mdgpu_unitcell_t* first_cell, bool need_host_staging, const FitFrames* fit = nullptr) {
     std::lock_guard<std::mutex> guard(p->slot_mutex);   // concurrent callers: the first one builds the slots
     if (p->slots.empty()) {
-        // default cell capacity: twice the grid the reference would build for the first frame, per property cutoff
+        // default cell capacity: twice the grid the reference would build for the first frame, per property cutoff. A non-periodic axis takes
+        // its extent from the data (AABB fit): with host frames that is the box of all the evaluation's frames (a superset of every
+        // property's points, so no frame of it needs more cells); frames on the device or in XTC blobs are not seen here, and get the floor.
         uint32_t cap = p->cell_cap;
         if (!cap) {
-            uint64_t need = 1u << 16;   // floor: non-periodic axes get their extent from the data (AABB fit), unknown here
+            float box[6]; const float* aabb = nullptr;
+            if (fit && (first_cell->flags & MDGPU_CELL_PBC_ALL) != MDGPU_CELL_PBC_ALL) { fit_frames_aabb(*fit, p->num_atoms, box); aabb = box; }
+            uint64_t need = 1u << 16;   // floor: room for later frames that spread beyond the first evaluation's
             auto grid = [&](double cell_ext, float cutoff) {
-                FrameGeom g; host_frame_geom(&g, first_cell, cell_ext, cutoff, nullptr, 0xffffffffu);
+                FrameGeom g; host_frame_geom(&g, first_cell, cell_ext, cutoff, aabb, 0xffffffffu);
                 need = std::max<uint64_t>(need, 2ull * std::max<uint64_t>(g.num_cells, g.num_home) + 2);
             };
             for (auto& pr : p->props) {
@@ -1648,7 +1664,8 @@ static int eval_host_frames_1(mdgpu_plan* p, const float* h_xyz, size_t frame_st
                               const mdgpu_unitcell_t* cells, size_t cell_stride_bytes, uint32_t frame_beg, uint32_t count) {
     CUDA_TRY(cudaSetDevice(p->device));
     if (!count) return 0;
-    int rc = ensure_slots(p, cell_at(cells, cell_stride_bytes, 0), true); if (rc) return rc;
+    const FitFrames fit{ h_xyz, frame_stride, axis_stride, count };
+    int rc = ensure_slots(p, cell_at(cells, cell_stride_bytes, 0), true, &fit); if (rc) return rc;
     cudaPointerAttributes attr{}; bool pinned = false;
     if (cudaPointerGetAttributes(&attr, h_xyz) == cudaSuccess) pinned = (attr.type == cudaMemoryTypeHost); else cudaGetLastError();
     const Space sp = p->ingest_space(); const bool c = sp == SPACE_COMPACT;
