@@ -129,6 +129,8 @@ typedef enum mdgpu_op {
  *              If ref_within_radius > 0 the reference argument was the dynamic selection within(radius, selection): idx[0] holds that
  *              selection and the references of a frame are the atoms of the system within `radius` of it, itself excluded (:2485-2533).
  *   SDF      : idx[0] = num_structures * structure_size atoms (equivalent structures), idx[1] = target atoms, cutoff_max.
+ *              Each structure's row of structure_size atoms must be strictly ascending (an atom set, as the reference's bitfields give it):
+ *              mdgpu_plan_create fails with MDGPU_ERR_INVALID_ARG for a row that is not, repeated atoms included.
  *   DENSITY_*: idx[0] = atoms.
  *   DISTANCE_MIN/_MAX: idx[0], idx[1] = the atoms of the two selections (brute force over all pairs, md_util_min_distance md_util.c:8242).
  *   DISTANCE_PAIR: an argument that was an ARRAY of selections contributes one position per selection, its centre of mass as for rdf's group references (extract_com :857): groups of
@@ -448,7 +450,8 @@ int mdgpu_plan_secondary_structure(mdgpu_plan* plan, size_t prop, uint32_t frame
 /* Exact integer results (what parity is asserted on).
  *  _counts: accumulated counts over all evaluated frames: RDF 1024 x u64 bins; SDF 128^3 x u64 voxels (widened from u32);
  *           DENSITY 1024 x u64 fixed-point mass sums (unit 2^-24 Da).
- *  _frame_counts: raw bins of one frame (needs keep_frame_results), RDF: u32[1024] plus the frame's pair total. */
+ *  _frame_counts: raw bins of one frame (needs keep_frame_results), RDF: u32[1024] plus the frame's pair total; SDF: the frame's hit total
+ *           (the voxel increments of all its structures) only, out_bins must be NULL. */
 int mdgpu_plan_property_counts(mdgpu_plan* plan, size_t prop, uint64_t* out, size_t out_len);
 int mdgpu_plan_property_frame_counts(mdgpu_plan* plan, size_t prop, uint32_t frame, uint32_t* out_bins, uint64_t* out_total);
 

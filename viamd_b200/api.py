@@ -339,6 +339,9 @@ def rdf_com(name, groups, trg_idx, cutoff, cutoff_min=0.0):
 
 
 def sdf(name, structures, trg_idx, cutoff):
+    """sdf(): structures is [num_structures, structure_size] atom indices, each row strictly ascending (an atom set, as the reference's
+    bitfields give it; Plan() raises MdgpuError for a row that is not, repeated atoms included). Row 0 of the initial frame is the
+    reference orientation; the target atoms are counted in a 128^3 volume around each structure, its own atoms excluded."""
     s = np.ascontiguousarray(structures, np.int32)
     assert s.ndim == 2, "structures: [num_structures, structure_size] atom indices"
     rng = {}; idx, dyn = _split_dyn([s.reshape(-1), trg_idx], rng)

@@ -719,6 +719,14 @@ mdgpu_plan* mdgpu_plan_create_ex(const mdgpu_system_desc_t* sys, const mdgpu_pro
         case MDGPU_OP_SDF: {
             if (!pr.n_struct || !pr.struct_size || pr.h_idx[0].size() != pr.n_struct * pr.struct_size)
                 return bail(MDGPU_ERR_INVALID_ARG, "sdf '" + pr.name + "': reference structures must be num_structures x structure_size atoms");
+            // a structure is an atom set (the reference passes bitfields): k_sdf_scatter excludes its atoms as one run when the first and last
+            // index span exactly structure_size atoms, which holds for contiguous rows only if they are strictly ascending
+            for (size_t s = 0; s < pr.n_struct; ++s) {
+                const int32_t* row = pr.h_idx[0].data() + s * pr.struct_size;
+                for (size_t k = 1; k < pr.struct_size; ++k)
+                    if (row[k] <= row[k - 1])
+                        return bail(MDGPU_ERR_INVALID_ARG, "sdf '" + pr.name + "': the atoms of reference structure " + std::to_string(s) + " are not strictly ascending");
+            }
             if (pr.h_idx[1].empty() && !pr.dyn[1].on) return bail(MDGPU_ERR_INVALID_ARG, "sdf '" + pr.name + "': The supplied target bitfield is empty");
             if (p->conn_off.empty()) return bail(MDGPU_ERR_INVALID_ARG, "sdf '" + pr.name + "': Missing bond connectivity");   // md_util.c:8746
             std::vector<int2> pairs; build_unwrap_pairs(pairs, pr.struct_size, p->conn_off, p->conn_idx);
@@ -2235,7 +2243,8 @@ int mdgpu_plan_property_frame_counts(mdgpu_plan* p, size_t prop, uint32_t frame,
     if (!p || prop >= p->props.size() || frame >= p->num_frames) return fail(MDGPU_ERR_INVALID_ARG, "mdgpu_plan_property_frame_counts: invalid argument");
     int rc = mdgpu_plan_sync(p); if (rc) return rc;
     Prop& pr = p->props[prop];
-    if (pr.op != MDGPU_OP_RDF) return fail(MDGPU_ERR_UNSUPPORTED, "per-frame counts are kept for rdf properties only");
+    if (pr.op == MDGPU_OP_SDF && out_bins) return fail(MDGPU_ERR_UNSUPPORTED, "sdf '%s' keeps the per-frame hit total only, no bins", pr.name.c_str());
+    if (pr.op != MDGPU_OP_RDF && pr.op != MDGPU_OP_SDF) return fail(MDGPU_ERR_UNSUPPORTED, "per-frame counts are kept for rdf and sdf properties only");
     if (out_bins) {
         if (!pr.d_keep.get()) return fail(MDGPU_ERR_INVALID_ARG, "plan was created without keep_frame_results");
         CUDA_TRY(cudaMemcpy(out_bins, pr.d_keep.get() + (size_t)frame * MDGPU_DIST_BINS, sizeof(uint32_t) * MDGPU_DIST_BINS, cudaMemcpyDeviceToHost));
