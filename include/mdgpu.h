@@ -207,7 +207,11 @@ typedef enum mdgpu_op {
  *   DISTANCE/ANGLE/DIHEDRAL: idx[k] = the atoms of argument k (0-based). A single integer index is that atom's position; an
  *              argument that was a selection (bit k of com_args set, or more than one index) is its centre of mass as
  *              coordinate_extract_com evaluates it (:1717 -> md_util_com_compute md_util.c:8163: periodic cells use the
- *              trigonometric centre of mass _com_pbc_iw :7850, 8-lane float accumulation as in the AVX2 build). */
+ *              trigonometric centre of mass _com_pbc_iw :7850, 8-lane float accumulation as in the AVX2 build).
+ *              dihedral (and BACKBONE_ANGLES) bring each bond vector to its minimum image with the reference's subtract / add loop
+ *              (min_image_ortho md_util.c:8424, the zone reduction of min_image_triclinic :8360), uncapped: a bond vector of any number of box
+ *              lengths gives the reference's value. Where the reference's loop never ends (a step leaves the component unchanged: an infinite
+ *              component, or one so large that x - box == x) the loop stops and the frame's value is NaN. */
 /* A dynamic selection as an argument: within([radius_min:]radius_max, selection) [and static_selection] (_within_expl_flt / _frng
  * md_script_functions.inl:2485-2720, `and` :1975), evaluated per frame on the device over the system-wide cell list (get_spatial_acc :734).
  * For argument k of a property, idx[k] holds the atoms of the within() selection and dyn[k] the rest.

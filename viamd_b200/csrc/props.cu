@@ -216,6 +216,25 @@ void launch_arg_com_parts(const BatchFrames& fr, const mdgpu_unitcell_t* d_cells
     note_launch("k_arg_com_parts", s);
 }
 
+// One subtract / add loop of min_image_ortho (md_util.c:8424-8436) or of min_image_triclinic's zone reduction (:8360-8423): while
+// d[i] > half subtract row `step` (components 0..i), then while d[i] <= -half add it, every step rounded as the reference rounds it.
+// There is no iteration cap, so every input on which the reference's loop ends gives its result, however many box lengths d[i] spans.
+// The reference never ends when a step leaves d[i] unchanged (d[i] infinite, or so large that d[i] - step[i] == d[i]); here the loop stops
+// there and returns false, and the caller makes the frame's value NaN. NaN input skips both loops, as in the reference.
+MDG_D bool min_image_loop(float* d, const float* step, int i, float half) {
+    while (d[i] > half) {
+        const float next = __fsub_rn(d[i], step[i]);
+        if (next == d[i]) return false;
+        for (int j = i; j >= 0; --j) d[j] = __fsub_rn(d[j], step[j]);
+    }
+    while (d[i] <= -half) {
+        const float next = __fadd_rn(d[i], step[i]);
+        if (next == d[i]) return false;
+        for (int j = i; j >= 0; --j) d[j] = __fadd_rn(d[j], step[j]);
+    }
+    return true;
+}
+
 // distance / angle / dihedral on the argument positions: an atom's coordinates (single index, coordinate_extract_com :1755) or the
 // centre of mass k_arg_com left in a.pos
 // distance (:3851-3890) / angle (:4099-4114) / dihedral (:4171-4196) of up to four positions in one cell
@@ -236,11 +255,10 @@ MDG_D float temporal_value(int op, const float P[4][3], const mdgpu_unitcell_t& 
         for (int k = 0; k < 3; ++k) for (int i = 0; i < 3; ++i) dx[k][i] = P[k + 1][i] - P[k][i];
         if (uc.flags & MDGPU_CELL_ORTHO) {   // min_image_ortho md_util.c:8424-8436
             for (int k = 0; k < 3; ++k) for (int i = 0; i < 3; ++i) {
-                const float half = ext[i] * 0.5f;
                 if (ext[i] > 0.0f) {
-                    int guard = 0;
-                    while (dx[k][i] > half && guard++ < 64) dx[k][i] -= ext[i];
-                    while (dx[k][i] <= -half && guard++ < 128) dx[k][i] += ext[i];
+                    float d = dx[k][i];
+                    if (!min_image_loop(&d, &ext[i], 0, __fmul_rn(ext[i], 0.5f))) return __int_as_float(0x7fffffff);
+                    dx[k][i] = d;
                 }
             }
         }
@@ -248,11 +266,8 @@ MDG_D float temporal_value(int op, const float P[4][3], const mdgpu_unitcell_t& 
             float box[3][3]; cell_box(uc, box);
             const float half3[3] = { box[0][0] * 0.5f, box[1][1] * 0.5f, box[2][2] * 0.5f };
             for (int k = 0; k < 3; ++k) {
-                for (int i = 2; i >= 0; --i) if (half3[i] > 0.0f) {
-                    int guard = 0;
-                    while (dx[k][i] > half3[i] && guard++ < 64) for (int j = i; j >= 0; --j) dx[k][j] = __fsub_rn(dx[k][j], box[i][j]);
-                    while (dx[k][i] <= -half3[i] && guard++ < 128) for (int j = i; j >= 0; --j) dx[k][j] = __fadd_rn(dx[k][j], box[i][j]);
-                }
+                for (int i = 2; i >= 0; --i)
+                    if (half3[i] > 0.0f && !min_image_loop(dx[k], box[i], i, half3[i])) return __int_as_float(0x7fffffff);
                 min_image_triclinic(dx[k], box);
             }
         }
